@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Benchmark of the accelerated path (driver contract: one JSON line on stdout).
 
-    python bench.py --gpus N --steps K --warmup W            # jiminy_b200 on N B200s of one node
+    python bench.py --gpus N --steps K --warmup W            # jiminy_b200 on N GPUs (H100) of one node
     python bench.py --impl reference --steps K --warmup W    # the CPU restatement of the reference path
 
 A "step" is one `Engine::step(0.04)` of every env of the batch -- for the default workload 4096
@@ -9,6 +9,7 @@ PD-controlled ANYmal envs per GPU with spring-damper ground contact, RK4 at dtMa
 dynamics evaluations + 8 derivative repairs + 41 stepper iterations per env-step), fp64.
 `value` is env-steps/s with actions already resident in HBM; `e2e` goes through the public C ABI
 with host buffers (pinned host actions -> H2D, step, sensor matrix D2H) every step.
+`--dump-outputs DIR` writes what the last timed step returned (t, q, v, a, sensors of every env) as DIR/<name>.npy.
 """
 import argparse
 import json
@@ -32,17 +33,18 @@ def read_peaks():
     if os.path.exists(path):
         with open(path) as fh:
             return json.load(fh), "measured"
-    return {"hbm_gbs": 6650.0}, "fallback"
+    return {"hbm_gbs": 3350.0}, "datasheet (H100 SXM)"
 
 
 class ClockSampler(threading.Thread):
-    """SM clock / throttle reasons / power during the timed region (B200_PROFILING.md's clocks line), polled through
+    """SM clock / throttle reasons / power during the timed region, polled through
     NVML every 5 ms (nvidia-smi itself needs ~100 ms per sample, longer than a short timed region); falls back to
     `nvidia-smi -lms` when pynvml is unavailable."""
 
     def __init__(self, index: int):
         super().__init__(daemon=True)
         self.index, self.samples, self._stop_evt, self.proc = index, [], threading.Event(), None
+        self.power_limit_w = None
 
     def _run_nvml(self) -> bool:
         try:
@@ -54,6 +56,7 @@ class ClockSampler(threading.Thread):
             except Exception:
                 h = nv.nvmlDeviceGetHandleByIndex(self.index)
             mx = nv.nvmlDeviceGetMaxClockInfo(h, nv.NVML_CLOCK_SM)
+            self.power_limit_w = nv.nvmlDeviceGetEnforcedPowerLimit(h) / 1000.0
         except Exception:
             return False
         bits = {"hw_slowdown": nv.nvmlClocksThrottleReasonHwSlowdown,
@@ -95,7 +98,7 @@ class ClockSampler(threading.Thread):
         if self.proc is not None:
             self.proc.terminate()
         self.join(timeout=1.0)
-        out = {"sm_mhz": None, "sm_max_mhz": None, "reasons": [], "samples": len(self.samples)}
+        out = {"sm_mhz": None, "sm_max_mhz": None, "power_limit_w": self.power_limit_w, "reasons": [], "samples": len(self.samples)}
         try:
             sm = [float(s[0]) for s in self.samples if len(s) >= 7]
             if sm:
@@ -202,6 +205,24 @@ def run_reference(args):
     print(json.dumps(line))
 
 
+DUMP_MAX_BYTES = 64 * 1024 * 1024
+
+
+def dump_outputs(out_dir, eng):
+    """What a caller of `BatchedEngine.step` receives after the last timed step: the state (t, q, v, a) and the sensor
+    matrix of every env, float64.  Above DUMP_MAX_BYTES the rows of a fixed, seeded sample of the envs (sorted)."""
+    t, q, v, a = eng.get_state()
+    outs = {"t": t, "q": q, "v": v, "a": a, "sensors": eng.get_sensors().copy()}
+    row_bytes = sum(x[:1].nbytes for x in outs.values())
+    budget = DUMP_MAX_BYTES - 4096                   # (room for the .npy headers)
+    if eng.n_env * row_bytes > budget:
+        keep = np.sort(np.random.default_rng(0).choice(eng.n_env, budget // row_bytes, replace=False))
+        outs = {k: x[keep] for k, x in outs.items()}
+    os.makedirs(out_dir, exist_ok=True)
+    for k, x in outs.items():
+        np.save(os.path.join(out_dir, f"{k}.npy"), np.ascontiguousarray(x, dtype=np.float64))
+
+
 def run_gpu(args):
     import torch
     import torch.distributed as dist
@@ -239,7 +260,7 @@ def run_gpu(args):
     xch = ObservationExchange(eng, rank, world, local_rank, prefer_peer=not args.nccl_gather)
     use_p2p = xch.mode == "peer"
     obs_gather = xch.note
-    flush = torch.empty(160 * 1024 * 1024 // 8, dtype=torch.float64, device=f"cuda:{local_rank}")  # > 126 MB L2
+    flush = torch.empty(160 * 1024 * 1024 // 8, dtype=torch.float64, device=f"cuda:{local_rank}")  # > 50 MB L2
 
     def barrier():
         if world > 1:
@@ -288,6 +309,8 @@ def run_gpu(args):
     eng.synchronize()       # PeerTimeout here = a signal of the timed region never arrived: no number is printed
     launches = eng.launch_count() - launches0
     clocks = sampler.stop()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, eng)     # before the arms below step the batch further
     kernel_ms = [a.elapsed_time(b) for (a, _), b in zip(ev, evk)]      # step kernel alone (roofline)
     step_ms = [a.elapsed_time(b) for a, b in ev]                        # step + observation all-gather
     step_ms_dev = float(np.mean(kernel_ms))
@@ -335,24 +358,6 @@ def run_gpu(args):
     e2e_value = total_envs * args.steps / (e2e_ms * 1e-3)
     peaks, peak_kind = read_peaks()
     bytes_per_launch = sc.algorithmic_bytes_per_env_step() * n_env
-    # `traffic` and the FP64-pipe figure come from the committed ncu capture of THIS device code (profiles/ncu_traffic.json is
-    # written by tools/ncu_traffic.py with the hash of jiminy_b200/csrc): a stale capture reports null, never an old number
-    traffic, fp64_pct, prof_src, stale_capture = None, None, None, None
-    try:
-        with open(os.path.join(ROOT, "profiles", "ncu_traffic.json")) as fh:
-            default = (args.contact_model in (None, "spring_damper") and args.ode_solver is None and args.dt_max is None and
-                       args.action == "pd" and args.flagged_fraction == 0.0)
-            rec = json.load(fh).get(args.workload) if default else None
-        if rec and rec["n_env"] == n_env and rec.get("kernel_source_sha") == kernel_source_sha():
-            traffic, fp64_pct, prof_src = rec["traffic_bytes"], rec["fp64_pipe_active_pct"], rec.get("source")
-        elif rec and rec["n_env"] == n_env:
-            # the device sources changed since the capture: the figures above stay null; what the last capture of this
-            # workload measured is reported apart, labelled with the device code it belongs to
-            stale_capture = {"traffic": rec["traffic_bytes"], "fp64_pipe_active_pct": rec["fp64_pipe_active_pct"],
-                             "ncu_capture": rec.get("source"), "kernel_source_sha": rec.get("kernel_source_sha"),
-                             "note": "taken on an earlier version of the device sources (hash above), not on the code timed here"}
-    except Exception:
-        pass
     achieved_gbs = bytes_per_launch / (step_ms_dev * 1e-3) / 1e9
     # supplementary (never the reported metric): the same steps back to back WITHOUT the L2 flush -- what a rollout loop
     # that does nothing else between two steps sees; for the small configs the cold misses of the flushed timing are most of it
@@ -376,6 +381,7 @@ def run_gpu(args):
         "ms_per_step": t_path_ms / args.steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
         "dtype": "f64", "data": "synthetic",
         "config": {"workload": workload_name(args, sc), "scenario": sc.description, "envs_total": total_envs, "lane_plan": eng.describe(),
+                   "gpu": torch.cuda.get_device_name(local_rank),
                    "l2": "160 MB buffer rewritten between timed steps (flush)", "ms_per_step_warm_l2_back_to_back": warm_ms, "obs_all_gather_ms": gather_ms, "obs_exchange": obs_gather,
                    "envs_failed": n_bad, "envs_flagged": n_bounds, "timed_region_wall_ms": wall_ms},
         "clocks": clocks,
@@ -383,13 +389,11 @@ def run_gpu(args):
                 "d2h_bytes_per_step": int(n_env * width * 8 * world), "ms_per_step": e2e_ms / args.steps},
         "gpu_launches": int(launches),
         "roofline": {"bound": "hbm", "achieved": achieved_gbs, "peak": peaks["hbm_gbs"], "unit": "GB/s",
-                     "frac": achieved_gbs / peaks["hbm_gbs"], "traffic": traffic, "peak_kind": peak_kind,
-                     "fp64_pipe_active_pct_ncu": fp64_pct, "ncu_capture": prof_src, "kernel_source_sha": kernel_source_sha(),
-                     "last_capture": stale_capture,
+                     "frac": achieved_gbs / peaks["hbm_gbs"], "peak_kind": peak_kind, "kernel_source_sha": kernel_source_sha(),
                      "kernel": "env_step_kernel", "kernel_ms": step_ms_dev,
                      "algorithmic_bytes_per_launch": bytes_per_launch,
                      "note": "fp64-pipe / latency bound by construction (state stays on chip for the whole "
-                             "env-step): see fp64 figures in DESIGN.md and profiles/"},
+                             "env-step): the HBM fraction is far below 1 by design"},
     }
     if cpu is not None:
         line["cpu_baseline"] = {"value": cpu["all_threads"]["value"], "unit": UNIT, "cores": ncores, "kind": "port",
@@ -422,7 +426,12 @@ def main():
     ap.add_argument("--flagged-fraction", type=float, default=0.0,
                     help="PD mode: share of the envs driven through their hip joint bounds (stepped by the full body with joint-bound constraints)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step returned (t, q, v, a, sensors; float64) as DIR/<name>.npy; "
+                         "beyond 64 MB, a fixed seeded sample of the envs")
     args = ap.parse_args()
+    if args.steps < 1 or args.warmup < 0:
+        ap.error("--steps must be >= 1 and --warmup >= 0")
     if args.impl == "reference":
         run_reference(args)
     else:

@@ -1,4 +1,4 @@
-/* jiminy_b200 -- C ABI of the B200-native batched rigid-body stepping library.
+/* jiminy_b200 -- C ABI of the H100-native batched rigid-body stepping library.
  *
  * This header is the drop-in boundary for ONE path of duburcqa/jiminy: the per-step rigid-body
  * pipeline of `jiminy::Engine::step` (core/src/engine/engine.cc:1724-2417) and the ODE
@@ -162,7 +162,7 @@ typedef struct JbSensorLayout {
 /* Message of the last failing call on this thread. */
 const char* jb_last_error(void);
 
-/* Library / build identification ("jiminy_b200 <ver> sm_100a"). */
+/* Library / build identification ("jiminy_b200 <ver> sm_90a"). */
 const char* jb_version(void);
 
 /* Engine option defaults, engine.h:260-341 (SURVEY.md App. D). */

@@ -231,7 +231,7 @@ static int launch(JbBatch* b, int mode, double step_dt, const uint8_t* d_mask = 
 extern "C" {
 
 const char* jb_last_error(void) { return g_err.c_str(); }
-const char* jb_version(void) { return "jiminy_b200 0.1 (sm_100a, fp64 lane-planned ABA)"; }
+const char* jb_version(void) { return "jiminy_b200 0.1 (sm_90a, fp64 lane-planned ABA)"; }
 
 void jb_default_options(JbOptions* o) {
     std::memset(o, 0, sizeof *o);

@@ -307,8 +307,8 @@ __device__ __noinline__ bool cons_solve_quadruped_t(const Ctx c, int* status) {
     };
     // The sweep is run some forty times per solve and what it costs is instruction fetch: straight-line code beyond the
     // 6 KB L0 instruction cache of the scheduler is delivered at ~45 cycles per 128-byte line, every iteration again
-    // (profiles/r02_constraint_path_investigation.txt: 6.7 k cycles per iteration for ~1.1 k instructions when the twelve
-    // updates of an iteration were unrolled, each in its own divergent region).  So the loops over the contacts are real
+    // (an earlier version unrolled the twelve updates of an iteration, each in its own divergent region, and paid about
+    // six cycles per instruction).  So the loops over the contacts are real
     // loops, the owner of a contact is a predicate, not a branch, and the relaxation schedule is a table: a few hundred
     // instructions that stay in the L0 for the whole solve.
     const int lane0 = c.lane - c.sub;

@@ -1,10 +1,10 @@
-// Device code of the batched rigid-body step (sm_100a, fp64).
+// Device code of the batched rigid-body step (sm_90a, fp64).
 //
 // One warp = 32/L environments; the L lanes of an env walk the lane plan of jb_plan.h.  All
 // per-env working data lives in shared memory as `field-major x 32 lanes` (conflict-free 8-byte
 // accesses), the hot per-joint quantities of a sweep live in registers and are carried from one
 // record to the next.  The reference functions each block replaces are cited inline
-// (paths relative to /root/reference).
+// (paths relative to the reference's source tree).
 #pragma once
 #ifdef JB_HOST_EMUL
 #include "jb_emul_shim.h"   // tests/emul: CPU thread emulation of a warp (test infrastructure only)

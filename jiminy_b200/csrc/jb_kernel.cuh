@@ -706,7 +706,7 @@ JB_DI unsigned int jb_smid() {
 __device__ __noinline__ void env_step_full(const LaunchArgs la, const bool only_flagged) {
     // constraint workspace of this block: one row per block of the launch.  (A pool of per-SM slots taken with an atomic
     // spin by lane 0 kept the workspace L2-resident, but left the warp's env groups running one after the other in the
-    // constraint solvers -- 3.7x on ANYmal with constraint contacts; profiles/r02_bisect_constraint_regression.txt.)
+    // constraint solvers -- several times slower on ANYmal with constraint contacts.)
     if (threadIdx.x == 0) jb_cw_slot = static_cast<int>(blockIdx.x);
     __syncwarp();
     env_step_body<false>(la, only_flagged);

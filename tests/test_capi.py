@@ -27,7 +27,7 @@ def test_header_symbols_exported():
     assert not missing, missing
     assert sorted(core.Api.SYMBOLS) == names      # the Python binding covers the whole header
     api = core.api()
-    assert b"sm_100a" in api.dll.jb_version()
+    assert b"sm_90a" in api.dll.jb_version()
 
 
 def test_default_options_match_reference_defaults():

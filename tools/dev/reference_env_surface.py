@@ -6,7 +6,7 @@ env configs load unchanged") for
   * the attributes they read on `jiminy_py.core` (alias `jiminy`) and `pinocchio` (alias `pin`),
   * the attributes they read on the engine / simulator / robot / state objects,
 checked against jiminy_b200's single-env `Engine` facade, `RobotTable`, `StepperState` and `RobotState`.  Reads
-/root/reference (this container only); the report it prints is committed under profiles/.
+the reference's sources (REF below); the report it prints is committed under profiles/.
 """
 import ast
 import importlib.util

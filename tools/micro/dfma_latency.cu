@@ -1,6 +1,6 @@
 // Microbenchmark: FP64 FMA issue cost per warp as a function of ILP (independent chains per thread)
 // and warps per SM sub-partition.  Answers: what instruction latency must a 1-warp-per-scheduler
-// kernel hide?   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o dfma_latency dfma_latency.cu
+// kernel hide?   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o dfma_latency dfma_latency.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 template <int ILP>

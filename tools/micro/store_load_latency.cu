@@ -1,6 +1,6 @@
 // Micro-benchmark behind the memory placement of the constraint solvers (DESIGN.md section 4): what does one thread
 // of a lone warp pay to re-read a value it has just stored, in global / local / shared memory?
-// Build + run: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o /tmp/store_load_latency tools/micro/store_load_latency.cu && /tmp/store_load_latency
+// Build + run: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o /tmp/store_load_latency tools/micro/store_load_latency.cu && /tmp/store_load_latency
 #include <cstdio>
 #include <cuda_runtime.h>
 __device__ __forceinline__ double ldg_(const double* p) { double v; asm volatile("ld.global.f64 %0, [%1];" : "=d"(v) : "l"(p) : "memory"); return v; }
