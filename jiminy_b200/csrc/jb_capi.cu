@@ -270,6 +270,8 @@ static int check_options(const JbOptions* o) {
 
 static void apply_options(JbBatch* b, const JbOptions* o) {
     b->kp.opt = *o;
+    b->kp.contact_inv_vt = 1.0 / o->contact_transition_velocity;
+    b->kp.contact_blend_k = o->contact_transition_eps > D_EPS ? -2.0 / o->contact_transition_eps : 0.0;
     double supd = INFINITY;
     if (o->sensors_update_period > 2.3e-16) supd = std::min(supd, o->sensors_update_period);
     if (o->controller_update_period > 2.3e-16) supd = std::min(supd, o->controller_update_period);
@@ -407,6 +409,7 @@ int jb_batch_create(const JbModelDesc* m, const JbOptions* opt, int32_t n_env, i
 
     if (SigQuadruped::matches(kp) && !std::getenv("JB_NO_STATIC_PLAN")) kp.sig_id = SigQuadruped::ID;
     kp.rhs_variant = (std::getenv("JB_QUADRUPED_ABA") && std::atoi(std::getenv("JB_QUADRUPED_ABA"))) ? 0 : 1;
+    kp.quad_stage = (kp.rhs_variant == 1 && !(std::getenv("JB_QUADRUPED_STAGE") && !std::atoi(std::getenv("JB_QUADRUPED_STAGE")))) ? 1 : 0;
     kp.fast_bounds = 0;   // set below, once the constraint tables exist
     // ---- constraint path: lookup tables, persistent state and workspace (jb_constraints.cuh)
     {
@@ -573,7 +576,7 @@ int jb_batch_create(const JbModelDesc* m, const JbOptions* opt, int32_t n_env, i
 int jb_describe(JbBatch* b, char* buf, int32_t len) {
     if (!b || !buf) return fail(JB_ERR_INVALID_ARGUMENT, "null argument");
     std::snprintf(buf, len, "%s; hot path: %s%s; constraints: %s", b->plan.describe().c_str(),
-                  b->kp.sig_id == SigQuadruped::ID ? (b->kp.rhs_variant == 1 ? "quadruped signature, composite-rigid-body evaluation" : "quadruped signature, ABA sweeps") : "ABA sweeps (dynamic plan)",
+                  b->kp.sig_id == SigQuadruped::ID ? (b->kp.rhs_variant == 1 ? (b->kp.quad_stage ? "quadruped signature, composite-rigid-body evaluation, one call per RK4 stage" : "quadruped signature, composite-rigid-body evaluation") :"quadruped signature, ABA sweeps") : "ABA sweeps (dynamic plan)",
                   b->kp.fast_bounds ? ", joint bounds solved in the evaluation" : "",
                   !b->kp.cons_on ? "flag only" : (b->kp.cq_on ? (b->kp.lb_on ? "structured quadruped solver + lane-block solver" : "structured quadruped solver + generic")
                                                  : (b->kp.bd_on ? "body-space contact solver + lane-block solver" : (b->kp.lb_on ? "lane-block solver" : "generic solver"))));

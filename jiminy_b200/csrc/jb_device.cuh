@@ -63,7 +63,10 @@ struct KParams {
     uint8_t kind_u[MAX_REC];       // lane-uniform record kind (0 = lanes differ)
     int32_t sig_id;                // static plan signature matched at batch creation (0 = none)
     int32_t rhs_variant;           // hot-path evaluation of the quadruped signature: 1 = composite-rigid-body form, 0 = ABA sweeps
-    int32_t fast_bounds;           // 1: joint position bounds are solved inside the hot-path evaluation (quadruped, composite form)
+    int32_t quad_stage;            // 1: an RK4 stage of the quadruped hot path is one call (stage_quadruped_crba), composite form only
+    double contact_inv_vt;         // 1 / contacts.transitionVelocity
+    double contact_blend_k;        // -2 / contacts.transitionEps, 0 when the blend is off (<= D_EPS)
+    int32_t fast_bounds;          // 1: joint position bounds are solved inside the hot-path evaluation (quadruped, composite form)
     int32_t uniform_solver;        // 1: full-mask collectives in the structured solver when the whole warp is in it
     double pgs_relax[100];         // relaxation factor of PGS iteration i (constraint_solvers.cc:236-248), tabulated by the host
     int32_t fast_bounds_io;        // (development) 0: skip the load / store of the bound state around the step
@@ -543,6 +546,18 @@ JB_DI V3 contact_dynamics(const JbOptions& o, double depth, V3 vw) {
     }
     return f;
 }
+// The same law without a branch, for a depth clamped to <= 0 (the caller selects the result by the sign of the unclamped
+// depth): the blend is a select on the host-computed -2 / transitionEps, the divisions are products with host-computed
+// reciprocals.  Finite for every finite input, depth 0 and zero sliding velocity included.
+JB_DI V3 contact_dynamics_nb(const JbOptions& o, double depth, V3 vw) {
+    const double vDepth = vw.z;
+    const double fN = -fmin(o.contact_stiffness * depth + o.contact_damping * vDepth, 0.0);
+    const double vRatio = fmin(sqrt(vw.x * vw.x + vw.y * vw.y) * KP->contact_inv_vt, 1.0);
+    const double fT = o.contact_friction * vRatio * fN;
+    const double bk = KP->contact_blend_k;
+    const double blend = bk != 0.0 ? tanh(depth * bk) : 1.0;
+    return mk(blend * (-fT * vw.x), blend * (-fT * vw.y), blend * fN);
+}
 
 // Motor constants the forward sweep needs, fetched at the top of a record (four 16-byte loads issued together with
 // the joint constants) so that their latency is hidden behind the kinematics instead of stalling computeEffort.
@@ -577,6 +592,16 @@ JB_DI void motor_effort_pre(const MotorConst& mc, const RecDbl* rd, int flags, d
         if (vj > 0.0) uTrans += rd->motor[4] * vj + rd->motor[6] * tanh(rd->motor[8] * vj);
         else uTrans += rd->motor[5] * vj + rd->motor[7] * tanh(rd->motor[8] * vj);
     }
+}
+// motor_effort_pre for flags 3 (effort limit and velocity taper, no friction) with the taper as a select, not a branch
+JB_DI void motor_effort_limited_nb(const MotorConst& mc, double cmd, double vj, double& uMotor, double& uTrans) {
+    const double vMotor = mc.red * vj;
+    const bool taper = mc.effLim * mc.invSlope > 0.0 && fabs(vMotor) > mc.thr;
+    const double kMin = fmin(fmax((mc.velLim + vMotor) * mc.invSpan, 0.0), 1.0);
+    const double kMax = fmin(fmax((mc.velLim - vMotor) * mc.invSpan, 0.0), 1.0);
+    const double eMin = taper ? -mc.effLim * kMin : -mc.effLim, eMax = taper ? mc.effLim * kMax : mc.effLim;
+    uMotor = fmin(fmax(cmd, eMin), eMax);
+    uTrans = mc.red * uMotor;
 }
 
 // SimpleMotor::computeEffort (core/src/hardware/basic_motors.cc:83-143)
@@ -1250,6 +1275,8 @@ JB_DI bool rhs_impl(const Ctx c, const bool up_to_date, int* status) {
 template <class BASE> struct FastOf : BASE { static constexpr bool fast_path = true; };
 template <class SIG, class = void> struct sig_is_fast { static constexpr bool value = false; };
 template <class BASE> struct sig_is_fast<FastOf<BASE>> { static constexpr bool value = true; };
+template <class SIG> struct is_fast_quadruped { static constexpr bool value = false; };
+template <> struct is_fast_quadruped<FastOf<SigQuadruped>> { static constexpr bool value = true; };
 constexpr int ENV_RETRY_FULL = 1 << 30;   // internal status bit, never stored
 
 // The three ABA sweeps are compiled once per plan signature, as out-of-line functions; the static one is a leaf
@@ -1466,11 +1493,90 @@ __device__ __noinline__ void bounds_solve_quadruped(const Ctx c, const bool up_t
     }
 }
 
-__device__ __noinline__ bool rhs_quadruped_crba(const Ctx c, const bool up_to_date, int* status) {
+// SE(3) integrate of the free-flyer, q1 = integrate(q0, dv), in quaternion form: the same map as integrate_free
+// (M1 = M0 exp6(v, w)) with the rotation composed as q0 (x) (sin(t/2) w / t, cos(t/2)), t = |w|, instead of building
+// exp6's rotation matrix and converting R0 Re back to a quaternion.  sin t = 2 s c and 1 - cos t = 2 s^2 come from one
+// jb_sincos(t / 2) (t / 2 is bounded by dt |w| / 2), 1 / t from one reciprocal square root; the Taylor branch of exp6
+// below TAYLOR_PREC3 is a select, so the whole integrate is one basic block.  Same sign continuity and first-order
+// normalisation as integrate_free.
+JB_DI void integrate_free_quat(const double* q0, const double* dv, double* q1) {
+    const V3 v = mk(dv[0], dv[1], dv[2]), w = mk(dv[3], dv[4], dv[5]);
+    const double t2 = dot(w, w);
+    const bool small = t2 < TAYLOR_PREC3 * TAYLOR_PREC3;     // t < TAYLOR_PREC3 (a power of two: exact)
+    const double inv_t = rsqrt(t2);
+    double sh, ch;
+    jb_sincos(0.5 * (t2 * inv_t), &sh, &ch);
+    const double inv_t2 = inv_t * inv_t;
+    const double alpha_wxv = small ? 0.5 - t2 * (1.0 / 24.0) : (2.0 * sh * sh) * inv_t2;   // (1 - cos t) / t^2
+    const double alpha_v = small ? 1.0 - t2 * (1.0 / 6.0) : (2.0 * sh * ch) * inv_t;       // sin t / t
+    const double alpha_w = small ? 1.0 / 6.0 - t2 * (1.0 / 120.0) : (1.0 - alpha_v) * inv_t2;
+    const double kq = small ? 0.5 - t2 * (1.0 / 48.0) : sh * inv_t;                         // sin(t / 2) / t
+    const double cq = small ? 1.0 - t2 * 0.125 : ch;                                        // cos(t / 2)
+    const V3 pe = alpha_v * v + (alpha_w * dot(w, v)) * w + alpha_wxv * cross(w, v);
+    double R0[9];
+    quat_to_R(q0[3], q0[4], q0[5], q0[6], R0);
+    const V3 p1 = mk(q0[0], q0[1], q0[2]) + rmul(R0, pe);
+    const double qe[4] = {kq * w.x, kq * w.y, kq * w.z, cq};
+    double q[4];
+    quat_mul(q0 + 3, qe, q);
+    const double dp = q[0] * q0[3] + q[1] * q0[4] + q[2] * q0[5] + q[3] * q0[6];
+    const double sg = dp < 0.0 ? -1.0 : 1.0;
+    const double N2 = q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3];
+    const double alpha = sg * ((3.0 - N2) / 2.0);
+    q1[0] = p1.x; q1[1] = p1.y; q1[2] = p1.z;
+    q1[3] = q[0] * alpha; q1[4] = q[1] * alpha; q1[5] = q[2] * alpha; q1[6] = q[3] * alpha;
+}
+
+// Evaluation of the quadruped signature in composite-rigid-body form.  STAGE = false: at the stage state already in
+// QS / VS.  STAGE = true: one whole Runge-Kutta stage -- forms the stage state QS = integrate(Q, wq kv), VS = V + wq ka
+// (kv / ka read at the field offsets kv1 / ka1 of the 1-dof records and kvf / kaf of the free-flyer), evaluates there
+// and adds wb (VS, A) to the accumulators (SV, SA) when wb != 0.  The stage state is kept in registers, the contact and
+// the springs take no branch: the base's integrate, the legs' position-only terms and the velocity pass form one basic
+// block that the scheduler interleaves.
+template <bool STAGE>
+JB_DI bool quadruped_crba(const Ctx c, const bool up_to_date, int* status, const double wq, const int kv1, const int ka1,
+                          const int kvf, const int kaf, const double wb) {
     using SIG = SigQuadruped;
     constexpr int L = 4;
     const JbOptions& opt = KP->opt;
     bool out_any = false;
+    double qb[7], vb[6], ql[4], vl[4];      // stage state of the free-flyer and of legs records 1..3
+    double spk[4] = {0, 0, 0, 0}, spd[4] = {0, 0, 0, 0};
+    if constexpr (STAGE) {
+        if (KP->springs != nullptr) {
+#pragma unroll
+            for (int r = 1; r < 4; ++r) {
+                const int iv = (KP->rint + (r * L + c.sub))->idx_v;
+                spk[r] = KP->springs[iv]; spd[r] = KP->springs[KP->nv + iv];
+            }
+        }
+        double* const rp = jb_smem + c.lane;
+        double q0[7], dv[6];
+#pragma unroll
+        for (int k = 0; k < 7; ++k) q0[k] = RP(RF_Q + k);
+#pragma unroll
+        for (int k = 0; k < 6; ++k) { dv[k] = wq * rp[(kvf + k) * 32]; vb[k] = RP(RF_V + k) + wq * rp[(kaf + k) * 32]; }
+        integrate_free_quat(q0, dv, qb);
+#pragma unroll
+        for (int k = 0; k < 7; ++k) RP(RF_QS + k) = qb[k];
+#pragma unroll
+        for (int k = 0; k < 6; ++k) RP(RF_VS + k) = vb[k];
+#pragma unroll
+        for (int r = 1; r < 4; ++r) {
+            double* const rq = jb_smem + SIG::rec_off(r) * 32 + c.lane;
+            ql[r] = rq[R1_Q * 32] + wq * rq[kv1 * 32];
+            vl[r] = rq[R1_V * 32] + wq * rq[ka1 * 32];
+            rq[R1_QS * 32] = ql[r]; rq[R1_VS * 32] = vl[r];
+        }
+    } else {
+        const double* const rp = jb_smem + c.lane;
+#pragma unroll
+        for (int k = 0; k < 7; ++k) qb[k] = RP(RF_QS + k);
+#pragma unroll
+        for (int k = 0; k < 6; ++k) vb[k] = RP(RF_VS + k);
+#pragma unroll
+        for (int r = 1; r < 4; ++r) { ql[r] = SMF(c, SIG::rec_off(r) + R1_QS); vl[r] = SMF(c, SIG::rec_off(r) + R1_VS); }
+    }
     // ======================= forward: kinematics, bias accelerations, bias forces, contact, motors ================
     Xf oMc; Mot vc, ac;
     {
@@ -1480,10 +1586,10 @@ __device__ __noinline__ bool rhs_quadruped_crba(const Ctx c, const bool up_to_da
         double* const rp = jb_smem + c.lane;   // record 0 starts at field 0
         Xf li;
         double Rq[9];
-        quat_to_R(RP(RF_QS + 3), RP(RF_QS + 4), RP(RF_QS + 5), RP(RF_QS + 6), Rq);
+        quat_to_R(qb[3], qb[4], qb[5], qb[6], Rq);
         mat3mul(K.placement, Rq, li.R);
-        li.p = ld3(K.placement + 9) + rmul(K.placement, mk(RP(RF_QS), RP(RF_QS + 1), RP(RF_QS + 2)));
-        const Mot v = sm_load_mot(c, RF_VS);
+        li.p = ld3(K.placement + 9) + rmul(K.placement, mk(qb[0], qb[1], qb[2]));
+        Mot v; v.l = mk(vb[0], vb[1], vb[2]); v.a = mk(vb[3], vb[4], vb[5]);
         Mot g0; g0.l = mk(-opt.gravity[0], -opt.gravity[1], -opt.gravity[2]); g0.a = mk(-opt.gravity[3], -opt.gravity[4], -opt.gravity[5]);
         const Mot a0 = motion_act_inv(li, g0);          // base acceleration at zero joint acceleration (v x vJ = 0 for the root)
         const double m = K.inertia[0];
@@ -1505,7 +1611,7 @@ __device__ __noinline__ bool rhs_quadruped_crba(const Ctx c, const bool up_to_da
         double* const rp = jb_smem + base * 32 + c.lane;
         const double sx = K.axis[0];
         double ca, sa;
-        jb_sincos(RP(R1_QS), &sa, &ca);
+        jb_sincos(ql[r], &sa, &ca);
         const double s = sx * sa;
         Xf li;
 #pragma unroll
@@ -1515,7 +1621,7 @@ __device__ __noinline__ bool rhs_quadruped_crba(const Ctx c, const bool up_to_da
             li.R[3 * i + 2] = ca * K.placement[3 * i + 2] - s * K.placement[3 * i + 1];
         }
         li.p = ld3(K.placement + 9);
-        const double qd = RP(R1_VS), w = sx * qd;
+        const double qd = vl[r], w = sx * qd;
         Xf oM;
         mat3mul(oMc.R, li.R, oM.R);
         oM.p = oMc.p + rmul(oMc.R, li.p);
@@ -1532,7 +1638,15 @@ __device__ __noinline__ bool rhs_quadruped_crba(const Ctx c, const bool up_to_da
             double* const cp = jb_smem + SIG::cslot_off() * 32 + c.lane;
             const V3 pc = ld3(ct->placement + 9);
             V3 Fl;
-            if (!up_to_date) {
+            if constexpr (STAGE) {
+                // evaluated whatever the depth, kept below the ground only
+                const V3 pos = oM.p + rmul(oM.R, pc);
+                const V3 vw = rmul(oM.R, v.l + cross(v.a, pc));
+                const V3 fc = rtmul(oM.R, contact_dynamics_nb(opt, fmin(pos.z, 0.0), vw));
+                const bool in = pos.z < 0.0;
+                Fl = mk(in ? fc.x : 0.0, in ? fc.y : 0.0, in ? fc.z : 0.0);
+                CO(0) = Fl.x; CO(1) = Fl.y; CO(2) = Fl.z;
+            } else if (!up_to_date) {
                 const V3 pos = oM.p + rmul(oM.R, pc);
                 Fl = mk(0, 0, 0);
                 if (pos.z < 0.0) {
@@ -1545,16 +1659,18 @@ __device__ __noinline__ bool rhs_quadruped_crba(const Ctx c, const bool up_to_da
             f.a = f.a - cross(pc, Fl);
         }
         double u = 0.0;
-        if (KP->springs != nullptr) {
+        if constexpr (STAGE) u = -spk[r] * ql[r] - spd[r] * qd;
+        else if (KP->springs != nullptr) {
             const int iv = (KP->rint + (r * L + c.sub))->idx_v;
-            u = -KP->springs[iv] * RP(R1_QS) - KP->springs[KP->nv + iv] * qd;
+            u = -KP->springs[iv] * ql[r] - KP->springs[KP->nv + iv] * qd;
         }
         double uM, uT;
-        motor_effort_pre(mc, rd, 3, RP(R1_CMD), qd, uM, uT);
+        if constexpr (STAGE) motor_effort_limited_nb(mc, RP(R1_CMD), qd, uM, uT);
+        else motor_effort_pre(mc, rd, 3, RP(R1_CMD), qd, uM, uT);
         RP(R1_UMOTOR) = uM;
         u += uT;
         RP(R1_U) = sx * u;                               // joint effort along the unsigned axis
-        if (!up_to_date) { const double qj = RP(R1_QS); out_any = out_any || K.q_hi < qj || qj < K.q_lo; }
+        if (!up_to_date) { const double qj = ql[r]; out_any = out_any || K.q_hi < qj || qj < K.q_lo; }
         sm_store_xf(c, base + R1_LIMI, li);
         sm_store_mot(c, base + R1_FU, f);
         oMc = oM; vc = v; ac = a;
@@ -1715,7 +1831,31 @@ __device__ __noinline__ bool rhs_quadruped_crba(const Ctx c, const bool up_to_da
         if (jb_any(c, mine)) { bounds_solve_quadruped(c, up_to_date, status); out_any = false; }
     }
     jb_syncwarp(c);
+    if constexpr (STAGE) {
+        // Runge-Kutta accumulators: SV += wb VS, SA += wb A (A as the bound solver may have left it)
+        if (wb != 0.0) {
+            double* const rp = jb_smem + c.lane;
+#pragma unroll
+            for (int k = 0; k < 6; ++k) { RP(RF_SV + k) += wb * vb[k]; RP(RF_SA + k) += wb * RP(RF_A + k); }
+#pragma unroll
+            for (int r = 1; r < 4; ++r) {
+                double* const rq = jb_smem + SIG::rec_off(r) * 32 + c.lane;
+                rq[R1_SV * 32] += wb * vl[r];
+                rq[R1_SA * 32] += wb * rq[R1_A * 32];
+            }
+        }
+    }
     return out_any;
+}
+
+__device__ __noinline__ bool rhs_quadruped_crba(const Ctx c, const bool up_to_date, int* status) {
+    return quadruped_crba<false>(c, up_to_date, status, 0.0, 0, 0, 0, 0, 0.0);
+}
+// One Runge-Kutta stage of the quadruped hot path (make_stage + rhs_fast + the accumulator update of step_rk4_t) in one
+// call; see quadruped_crba.
+__device__ __noinline__ void stage_quadruped_crba(const Ctx c, const double wq, const int kv1, const int ka1, const int kvf,
+                                                  const int kaf, const double wb, int* status) {
+    if (quadruped_crba<true>(c, false, status, wq, kv1, ka1, kvf, kaf, wb)) *status |= ENV_RETRY_FULL;
 }
 
 // Engine::computeRobotsDynamics: the sweeps give the unconstrained accelerations; then the constraint path
@@ -1982,10 +2122,19 @@ __device__ __noinline__ void step_rk4_t(const Ctx c, double dt, int* status) {
             RP(R1_SA) = 0.0 + w * RP(R1_A);
         }
     });
+    constexpr bool quad_fast = is_fast_quadruped<SIG>::value;
+    const bool one_call = quad_fast && KP->quad_stage;
 #pragma unroll 1
     for (int i = 1; i < 4; ++i) {
         // stage state from k_{i-1}: kv_{i-1} is V (i == 1) or the previous stage velocity VS, ka_{i-1} is in A
         const double w = dt * (i == 3 ? 1.0 : 0.5);
+        if constexpr (quad_fast) {
+            if (one_call) {
+                stage_quadruped_crba(c, w, i == 1 ? R1_V : R1_VS, R1_A, i == 1 ? RF_V : RF_VS, RF_A,
+                                     dt * (i == 3 ? 1.0 / 6.0 : 1.0 / 3.0), status);
+                continue;
+            }
+        }
         if (i == 1) make_stage<SIG>(c, w, R1_V, R1_A, RF_V, RF_A);
         else make_stage<SIG>(c, w, R1_VS, R1_A, RF_VS, RF_A);
         rhs_sig<SIG>(c, false, status);
@@ -2006,7 +2155,12 @@ __device__ __noinline__ void step_rk4_t(const Ctx c, double dt, int* status) {
         });
     }
     // candidate solution = x0 (+) sum ; it is always accepted, then dx = f(t + dt, x)
-    make_stage<SIG>(c, 1.0, R1_SV, R1_SA, RF_SV, RF_SA);
+    if constexpr (quad_fast) {
+        if (one_call) stage_quadruped_crba(c, 1.0, R1_SV, R1_SA, RF_SV, RF_SA, 0.0, status);
+        else make_stage<SIG>(c, 1.0, R1_SV, R1_SA, RF_SV, RF_SA);
+    } else {
+        make_stage<SIG>(c, 1.0, R1_SV, R1_SA, RF_SV, RF_SA);
+    }
     SIG::for_each_forward([&](auto r_) {
         const int r = r_;
         const int kind = SIG::kind(r, c);
@@ -2023,7 +2177,7 @@ __device__ __noinline__ void step_rk4_t(const Ctx c, double dt, int* status) {
             RP(R1_V) = RP(R1_VS);
         }
     });
-    rhs_sig<SIG>(c, false, status);
+    if (!one_call) rhs_sig<SIG>(c, false, status);
 }
 
 // run-time dispatch on the plan signature

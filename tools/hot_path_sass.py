@@ -1,0 +1,105 @@
+#!/usr/bin/env python
+"""Static SASS summary of the quadruped hot path in the step kernel (env_step_kernel_t<true>): for the RK4 step of the
+quadruped signature, the composite-rigid-body evaluation and the one-call RK4 stage, print the instruction count, the
+FP64 instruction count, basic blocks, local-memory traffic (STL / LDL), calls into the library's division / square-root
+/ trigonometric slow paths, and the spills ptxas reports.
+
+Usage: python tools/hot_path_sass.py [--lib LIB.so [--ptxas-log LOG]]
+Without --lib the library is compiled from the tree into a temporary directory (with -Xptxas -v, for the spills).
+With --lib the spill column comes from --ptxas-log when given, else it is left out."""
+import argparse
+import collections
+import os
+import re
+import subprocess
+import sys
+import tempfile
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+KERNEL = "_ZN2jb17env_step_kernel_tILb1EEEvNS_10LaunchArgsE"
+FUNCS = [("step_rk4_t<FastOf<SigQuadruped>>", "_ZN2jb10step_rk4_tINS_6FastOfINS_13SigQuadrupedTILb0EEEEEEEvNS_3CtxEdPi"),
+         ("rhs_quadruped_crba", "_ZN2jb18rhs_quadruped_crbaENS_3CtxEbPi"),
+         ("stage_quadruped_crba", "_ZN2jb20stage_quadruped_crbaENS_3CtxEdiiiidPi")]
+FP64 = {"DFMA", "DMUL", "DADD", "DSETP", "DMNMX"}
+
+
+def build(tmp):
+    sys.path.insert(0, ROOT)
+    import __graft_entry__ as g
+    lib = os.path.join(tmp, "libjiminy_b200.so")
+    srcs = [os.path.join(g.CSRC, f) for f in ("jb_capi.cu", "jb_plan.cpp")]
+    r = subprocess.run([g._nvcc()] + g.NVCC_FLAGS + ["-Xptxas", "-v", "-o", lib] + srcs + ["-ccbin", "/usr/bin/g++"],
+                       capture_output=True, text=True, check=True)
+    return lib, r.stdout + r.stderr
+
+
+def spills(log):
+    out, cur = {}, None
+    for line in log.splitlines():
+        m = re.search(r"Function properties for (\S+)", line)
+        if m:
+            cur = m.group(1)
+            continue
+        m = re.search(r"(\d+) bytes spill stores, (\d+) bytes spill loads", line)
+        if m and cur:
+            out[cur] = int(m.group(1)) + int(m.group(2))
+            cur = None
+    return out
+
+
+def disassemble(lib, tmp):
+    subprocess.run(["cuobjdump", "-xelf", "all", os.path.abspath(lib)], cwd=tmp, check=True, capture_output=True)
+    cubin = max((os.path.join(tmp, f) for f in os.listdir(tmp) if f.endswith(".cubin")), key=os.path.getsize)
+    return subprocess.run(["nvdisasm", "-c", cubin], capture_output=True, text=True, check=True).stdout.splitlines()
+
+
+def body(lines, mangled):
+    head = f"${KERNEL}${mangled}:"
+    try:
+        start = lines.index(head)
+    except ValueError:
+        return None
+    end = next((i for i in range(start + 1, len(lines)) if re.match(r"^(\.text|\$\S+:$)", lines[i])), len(lines))
+    return lines[start + 1:end]
+
+
+def summary(fn):
+    ins = [l for l in fn if re.match(r"^\s+/\*[0-9a-f]{4,}\*/", l)]
+    op = [re.sub(r"^\s+/\*[0-9a-f]+\*/\s+(@!?U?P[T\d]\s+)?", "", l).split()[0].split(".")[0] for l in ins]
+    cnt = collections.Counter(op)
+    calls = collections.Counter(m.group(1) for l in ins for m in [re.search(r"CALL\S*\s+`\(\S*?(__internal[\w$]*)\)", l)] if m)
+    return {"instructions": len(ins), "fp64": sum(cnt[o] for o in FP64),
+            "basic_blocks": 1 + sum(1 for l in fn if re.match(r"^\.L_x_\d+:", l)),
+            "STL": cnt["STL"], "LDL": cnt["LDL"],
+            "slow_path_calls": sum(calls.values()),
+            "trig_calls": sum(v for k, v in calls.items() if "trig" in k),
+            "calls_by_target": dict(calls)}
+
+
+def main():
+    ap = argparse.ArgumentParser(description=__doc__.splitlines()[0])
+    ap.add_argument("--lib")
+    ap.add_argument("--ptxas-log")
+    a = ap.parse_args()
+    with tempfile.TemporaryDirectory() as tmp:
+        if a.lib:
+            lib, log = a.lib, (open(a.ptxas_log).read() if a.ptxas_log else None)
+        else:
+            lib, log = build(tmp)
+        lines = disassemble(lib, tmp)
+    sp = spills(log) if log is not None else {}
+    print(f"library: {lib}")
+    cols = ["instructions", "fp64", "basic_blocks", "STL", "LDL", "slow_path_calls", "trig_calls", "spill_bytes"]
+    print(f"{'function':<34}" + "".join(f"{c:>16}" for c in cols))
+    for name, mangled in FUNCS:
+        fn = body(lines, mangled)
+        if fn is None:
+            print(f"{name:<34}  (not in this library)")
+            continue
+        s = summary(fn)
+        s["spill_bytes"] = sp.get(mangled, "n/a")
+        print(f"{name:<34}" + "".join(f"{s[c]:>16}" for c in cols) + f"   {s['calls_by_target']}")
+
+
+if __name__ == "__main__":
+    main()
