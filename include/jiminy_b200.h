@@ -45,6 +45,8 @@ extern "C" {
 #define JB_ENV_CONTACT_FORCE 32   /* jb_start: initial contact force > 1e5 N (engine.cc:1338-1345)  */
 #define JB_ENV_SOLVER_FAILED 64   /* "Too many successive constraint solving failures" (engine.cc:2363-2372) */
 #define JB_ENV_CONSTRAINT_OVERFLOW 128 /* more constraint rows enabled at once than the batch was sized for */
+#define JB_ENV_BAD_START 256      /* jb_start_device: the env's (q0, v0) row failed Engine::start's input checks
+                                     (NaN, q out of bounds); set together with JB_ENV_NOT_STARTED          */
 
 /* ---------------------------------------------------------------- joint model types --- */
 /* Pinocchio 2.7 joint models produced by its URDF parser (SURVEY.md App. B). */
@@ -214,6 +216,13 @@ int jb_get_constraints(JbBatch* batch, uint8_t* joint_enabled, double* joint_lam
  * runs forward kinematics, the initial contact-force guard, the INIT_ITERATIONS fixed-point loop
  * and the first sensor refresh; sets t = 0, dt = SIMULATION_MIN_TIMESTEP. */
 int jb_start(JbBatch* batch, const uint8_t* mask, const double* q0, const double* v0);
+/* jb_start with device inputs of the same layouts (mask_dev may be NULL: all envs), enqueued on the batch stream without
+ * any host synchronisation: the caller keeps the buffers alive until the stream has passed the call.  The input checks
+ * of Engine::start run inside the kernel, per env: an env whose row holds a NaN, or a q outside [q_lower - eps,
+ * q_upper + eps] (eps = 2.22e-16, as jb_start), is not started -- its status word becomes JB_ENV_NOT_STARTED |
+ * JB_ENV_BAD_START and nothing else of it is written -- while the other envs start normally.  The generator start
+ * states of the sensor pipeline are recomputed on the host only after jb_set_seeds / jb_set_sensor_options. */
+int jb_start_device(JbBatch* batch, const uint8_t* mask_dev, const double* q0_dev, const double* v0_dev);
 
 /* Replaces: the command buffer written by AbstractController::computeCommand through the
  * FunctionalController callback (engine.cc:3240-3251; controller_functor.h:27-80).  The command is
@@ -239,6 +248,15 @@ int jb_set_pd_controller_full(JbBatch* batch, const double* kp, const double* kd
  * (:167-262, :620-640), which is what the getter and the setter are for.  Both need the block enabled. */
 int jb_get_pd_controller_state(JbBatch* batch, double* state);
 int jb_set_pd_controller_state(JbBatch* batch, const double* state);
+/* gym_jiminy's `PDAdapter` block (proportional_derivative_controller.py:166-262, :538-660) on the device, in front of
+ * the `PDController` block: jb_set_pd_adapter configures it (order 0: the action is the target motor position at the
+ * end of the env-step, 1: the target velocity; `velocity_deadband` [nmotors] or NULL); jb_pd_adapter_device then turns
+ * the device action `[n_env][nmotors]` into the target accelerations of the coming env-step -- the command buffer
+ * jb_set_command would fill -- reading, and in the instantaneous mode writing, the block's command state, with the
+ * bounds given to jb_set_pd_controller_full.  |step_dt| < 1e-9 writes zero accelerations and leaves the state alone.
+ * One small kernel on the batch stream, no host synchronisation; the step kernel is not involved. */
+int jb_set_pd_adapter(JbBatch* batch, int32_t order, int32_t is_instantaneous, const double* velocity_deadband);
+int jb_pd_adapter_device(JbBatch* batch, const double* action_dev, double step_dt);
 
 /* gym_jiminy's `MahonyFilter` observer on the device (blocks/mahony_filter.py:28-101, :337-393 with the default
  * exact_init = True, ignore_twist = False): the attitude estimate of every IMU starts from the true orientation of
@@ -359,6 +377,10 @@ int jb_get_iters(JbBatch* batch, int64_t* iter, int64_t* iter_failed);
  * matrix `[n_env][width]` and the stacked (q, v) `[n_env][nq+nv]`, refreshed by jb_step.  This
  * is the buffer a multi-GPU rollout all-gathers (SURVEY.md 8e). */
 int jb_device_views(JbBatch* batch, double** sensors_dev, double** qv_dev);
+/* The device buffers behind jb_get_status (`status` [n_env]), jb_get_pd_controller_state (`pd_state`
+ * [n_env][3][nmotors]) and jb_get_mahony_filter (`mahony` [n_env][nimu][10]), same layouts; a pointer is NULL when its
+ * block is off.  Any argument may be NULL.  Contents are those of the last launch that has completed on the batch stream. */
+int jb_device_block_views(JbBatch* batch, int32_t** status, double** pd_state, double** mahony);
 
 /* Model randomisation: `Model::addBiasedToExtendedModel` (core/src/robot/model.cc:1166-1236; options
  * `centerOfMassPositionBodiesBiasStd`, `massBodiesBiasStd`, `inertiaBodiesBiasStd`, `relativePositionBodiesBiasStd`)

@@ -23,6 +23,7 @@ JB_ERR_INVALID_ARGUMENT, JB_ERR_BAD_CONTROL_FLOW, JB_ERR_RUNTIME, JB_ERR_NOT_IMP
 JB_ERR_PEER_TIMEOUT = -6
 JB_ENV_OK, JB_ENV_NAN, JB_ENV_ITER_FAILED, JB_ENV_DT_UNDERFLOW = 0, 1, 2, 4
 JB_ENV_JOINT_LIMIT, JB_ENV_NOT_STARTED, JB_ENV_CONTACT_FORCE = 8, 16, 32
+JB_ENV_BAD_START = 256
 
 
 class BadControlFlow(RuntimeError):
@@ -62,7 +63,8 @@ class Api:
                "jb_set_pd_controller_full", "jb_set_mahony_filter", "jb_get_mahony_filter",
                "jb_get_pd_controller_state", "jb_set_pd_controller_state", "jb_get_constraints",
                "jb_get_stepper_state", "jb_set_stepper_state", "jb_get_centroidal",
-               "jb_set_sensor_options", "jb_set_seeds", "jb_get_sensor_data")
+               "jb_set_sensor_options", "jb_set_seeds", "jb_get_sensor_data",
+               "jb_start_device", "jb_set_pd_adapter", "jb_pd_adapter_device", "jb_device_block_views")
 
     def __init__(self, cdll: C.CDLL):
         self.dll = L = cdll
@@ -125,6 +127,10 @@ class Api:
         L.jb_peer_obs_wait.argtypes = [vp]
         L.jb_peer_obs_enable.argtypes = [vp, C.c_int32]
         L.jb_peer_obs_view.argtypes = [vp, C.POINTER(vp)]
+        L.jb_start_device.argtypes = [vp, vp, vp, vp]
+        L.jb_set_pd_adapter.argtypes = [vp, C.c_int32, C.c_int32, c_double_p]
+        L.jb_pd_adapter_device.argtypes = [vp, vp, C.c_double]
+        L.jb_device_block_views.argtypes = [vp, C.POINTER(vp), C.POINTER(vp), C.POINTER(vp)]
 
     def check(self, rc: int) -> None:
         if rc != JB_OK:
@@ -373,6 +379,32 @@ class BatchedEngine:
         self._api.check(self._api.dll.jb_start(self._h, None if m is None else m.ctypes.data_as(c_uint8_p),
                                                dptr(q0), dptr(v0)))
 
+    def start_device(self, q0_ptr: int, v0_ptr: int, mask_ptr: Optional[int] = None) -> None:
+        """`start` from device buffers (q0 [n_env, nq], v0 [n_env, nv] fp64, mask [n_env] uint8 or None = all), enqueued on
+        the batch stream with no host synchronisation: keep the buffers alive until the stream has passed the call.  Rows
+        that fail the input checks leave their env not started, with status JB_ENV_NOT_STARTED | JB_ENV_BAD_START."""
+        self._api.check(self._api.dll.jb_start_device(self._h, C.c_void_p(mask_ptr or None), C.c_void_p(q0_ptr),
+                                                      C.c_void_p(v0_ptr)))
+
+    def set_pd_adapter(self, order: int = 1, is_instantaneous: bool = False, velocity_deadband=None) -> None:
+        """Configures the device `PDAdapter` block in front of the `PDController` block (`set_pd_controller_full`)."""
+        db = None if velocity_deadband is None else \
+            np.ascontiguousarray(np.broadcast_to(np.asarray(velocity_deadband, dtype=np.float64), (self.nm,)))
+        self._api.check(self._api.dll.jb_set_pd_adapter(self._h, int(order), 1 if is_instantaneous else 0,
+                                                        None if db is None else dptr(db)))
+
+    def pd_adapter_device(self, action_ptr: int, step_dt: float) -> None:
+        """Device `PDAdapter` on the action buffer [n_env, nmotors] (fp64, device): the target accelerations of the
+        coming env-step go to the command buffer.  Asynchronous, on the batch stream."""
+        self._api.check(self._api.dll.jb_pd_adapter_device(self._h, C.c_void_p(action_ptr), float(step_dt)))
+
+    def device_block_views(self) -> Tuple[int, int, int]:
+        """Device pointers (status [n_env] int32, PD controller state [n_env, 3, nmotors], Mahony filter state
+        [n_env, nimu, 10]); 0 where the block is off."""
+        s, p, m = C.c_void_p(), C.c_void_p(), C.c_void_p()
+        self._api.check(self._api.dll.jb_device_block_views(self._h, C.byref(s), C.byref(p), C.byref(m)))
+        return s.value or 0, p.value or 0, m.value or 0
+
     def set_command(self, cmd) -> None:
         if not self.nm:
             return
@@ -518,6 +550,13 @@ class BatchedEngine:
                 "sensors": np.ctypeslib.as_array(hv.sensors, shape=(n, max(self.width, 1)))[:, :self.width],
             }
         return self._views
+
+    def device_state_ptrs(self) -> Dict[str, int]:
+        """Device pointers of `jb_state_ptrs`: t [n_env], qv [n_env, nq + nv], sensors [n_env, width] (env-major)."""
+        dv = JbStateViews()
+        self._api.check(self._api.dll.jb_state_ptrs(self._h, None, C.byref(dv)))
+        return {"t": C.cast(dv.t, C.c_void_p).value or 0, "qv": C.cast(dv.qv, C.c_void_p).value or 0,
+                "sensors": C.cast(dv.sensors, C.c_void_p).value or 0}
 
     def stream(self) -> int:
         s = C.c_void_p()

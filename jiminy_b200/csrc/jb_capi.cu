@@ -58,10 +58,16 @@ struct JbBatch {
     double* d_springs = nullptr;
     double *d_pd = nullptr, *d_cmd_torque = nullptr, *d_pdf = nullptr, *d_pdf_state = nullptr, *d_mahony = nullptr;
     double *d_pdf_snap = nullptr, *d_mahony_snap = nullptr;
+    double* d_qbounds = nullptr;   // [2][nq] q_lower, q_upper (input checks of jb_start_device)
+    // device PDAdapter (jb_set_pd_adapter)
+    int32_t ad_order = -1, ad_instantaneous = 0;
+    double* d_ad_deadband = nullptr;
+    bool ad_has_deadband = false;
     // sensor measurement pipeline (jb_set_sensor_options / jb_set_seeds)
     std::vector<SensorDesc> sdesc;
     std::vector<uint32_t> seeds;
     bool sp_dirty = false;
+    bool sp_rows_dirty = true;     // seeds or sensor set changed since every env's generator start state was uploaded
     int sp_cap_alloc = 0;
     SensorDesc* d_sdesc = nullptr;
     unsigned long long *d_sp_rng = nullptr, *d_sp_rng_init = nullptr, *d_sp_snap_rng = nullptr;
@@ -169,12 +175,13 @@ static int ensure_host_stage(JbBatch* b, size_t bytes) {
 static KParams g_kp_on_device[64];
 static bool g_kp_valid[64] = {};
 #endif
-static int launch(JbBatch* b, int mode, double step_dt, const uint8_t* d_mask = nullptr, const double* d_command = nullptr) {
+static int launch(JbBatch* b, int mode, double step_dt, const uint8_t* d_mask = nullptr, const double* d_command = nullptr,
+                  bool validate = false) {
     KParams kp = b->kp;
     // static plan signatures carry no external-force code
     if (kp.n_eslot > 0) kp.sig_id = 0;
     LaunchArgs la{};
-    la.mode = mode; la.step_dt = step_dt; la.mask = d_mask; la.command = d_command;
+    la.mode = mode; la.step_dt = step_dt; la.mask = d_mask; la.command = d_command; la.validate = validate ? 1 : 0;
     if (mode == MODE_STEP && b->peer_world > 1 && !b->peer_opened.empty() && b->peer_enabled) {
         ++b->step_id;
         la.peer_on = 1;
@@ -382,18 +389,21 @@ int jb_batch_create(const JbModelDesc* m, const JbOptions* opt, int32_t n_env, i
     ALLOC(b->d_springs, 2 * static_cast<size_t>(m->nv)); ALLOC(b->d_mask, n_env);
     ALLOC(b->d_pd, 2 * static_cast<size_t>(m->nmotors)); ALLOC(b->d_cmd_torque, static_cast<size_t>(n_env) * m->nmotors);
     ALLOC(b->d_stage, static_cast<size_t>(n_env) * std::max(std::max(m->nq, m->nv), SCH_N + 0));
+    ALLOC(b->d_qbounds, 2 * static_cast<size_t>(m->nq));
 #define ALLOC2 ALLOC
     cudaMemcpyAsync(d_rint, P.rint.data(), P.rint.size() * sizeof(RecInt), cudaMemcpyHostToDevice, b->stream);
     cudaMemcpyAsync(d_rdbl, P.rdbl.data(), P.rdbl.size() * sizeof(RecDbl), cudaMemcpyHostToDevice, b->stream);
     if (!P.cslots.empty()) cudaMemcpyAsync(d_cs, P.cslots.data(), P.cslots.size() * sizeof(ContactSlot), cudaMemcpyHostToDevice, b->stream);
     if (m->nimu) cudaMemcpyAsync(d_imu, m->imu_placement, 12 * sizeof(double) * m->nimu, cudaMemcpyHostToDevice, b->stream);
+    cudaMemcpyAsync(b->d_qbounds, b->q_lower.data(), sizeof(double) * m->nq, cudaMemcpyHostToDevice, b->stream);
+    cudaMemcpyAsync(b->d_qbounds + m->nq, b->q_upper.data(), sizeof(double) * m->nq, cudaMemcpyHostToDevice, b->stream);
     std::vector<int32_t> st(N, JB_ENV_NOT_STARTED);
     cudaMemcpyAsync(b->d_status, st.data(), N * sizeof(int32_t), cudaMemcpyHostToDevice, b->stream);
     kp.rint = d_rint; kp.rdbl = d_rdbl; kp.cslots = d_cs; kp.imu_placement = d_imu; kp.springs = nullptr;
     kp.pd_gains = nullptr; kp.cmd_torque = b->d_cmd_torque; kp.pdf = nullptr; kp.pdf_state = nullptr; kp.pdf_safety = 0; kp.mahony = nullptr; kp.mahony_kp = 1.0; kp.mahony_ki = 0.1;
     kp.q = b->d_q; kp.v = b->d_v; kp.a = b->d_a; kp.sched = b->d_sched; kp.iters = b->d_iters; kp.status = b->d_status;
     kp.command = b->d_cmd; kp.sensors = b->d_sensors; kp.qv_out = b->d_qv;
-    kp.q_in = b->d_qin; kp.v_in = b->d_vin;
+    kp.q_in = b->d_qin; kp.v_in = b->d_vin; kp.q_bounds = b->d_qbounds;
     kp.a_out = b->d_aout; kp.fext_out = b->d_fext; kp.u_out = b->d_u;
     kp.eff_u = b->d_u; kp.eff_umotor = b->d_umotor; kp.eff_fext = b->d_fext;
     {
@@ -725,6 +735,79 @@ int jb_set_pd_controller_state(JbBatch* b, const double* state) {
     return JB_OK;
 }
 
+// PDAdapter block (pd_adapter, proportional_derivative_controller.py:166-262) for one (env, motor): what
+// jiminy_b200/blocks.py:pd_adapter computes on the host, operation for operation (no contraction into FMAs), so that
+// both give the same bits.
+#ifdef JB_HOST_EMUL
+#define JB_MUL_RN(a, b) ((a) * (b))
+#define JB_ADD_RN(a, b) ((a) + (b))
+#else
+#define JB_MUL_RN(a, b) __dmul_rn((a), (b))
+#define JB_ADD_RN(a, b) __dadd_rn((a), (b))
+#endif
+// np.minimum(np.maximum(x, lo), hi), NaN propagating
+__device__ __forceinline__ double adapter_clip(double x, double lo, double hi) {
+    const double y = x < lo ? lo : x;
+    return y > hi ? hi : y;
+}
+
+__global__ void pd_adapter_kernel(const double* __restrict__ action, double* __restrict__ state, const double* __restrict__ pdf,
+                                  const double* __restrict__ deadband, double* __restrict__ out, int n_env, int nm, int order,
+                                  int instantaneous, double dt) {
+    const size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x;
+    if (i >= static_cast<size_t>(n_env) * nm) return;
+    const size_t env = i / nm;
+    const int m = static_cast<int>(i % nm);
+    if (fabs(dt) < 1e-9) { out[i] = 0.0; return; }
+    double* st = state + env * 3 * nm;
+    const double a = action[i];
+    if (instantaneous) {
+        if (order == 0) {
+            double velocity = adapter_clip((a - st[m]) / dt, pdf[3 * nm + m], pdf[6 * nm + m]);
+            if (deadband && fabs(velocity) < deadband[m]) velocity = 0.0;
+            st[m] = JB_ADD_RN(st[m], JB_MUL_RN(velocity, dt));
+            st[nm + m] = 0.0;
+        } else {
+            const double act = deadband ? a * (fabs(a) > deadband[m] ? 1.0 : 0.0) : a;
+            const double acceleration = adapter_clip((act - st[nm + m]) / dt, pdf[4 * nm + m], pdf[7 * nm + m]);
+            st[nm + m] = JB_ADD_RN(st[nm + m], JB_MUL_RN(acceleration, dt));
+        }
+        out[i] = 0.0;
+    } else {
+        double velocity = adapter_clip(order == 0 ? (a - st[m]) / dt : a, pdf[3 * nm + m], pdf[6 * nm + m]);
+        if (deadband && fabs(velocity) < deadband[m]) velocity = 0.0;
+        out[i] = (velocity - st[nm + m]) / dt;
+    }
+}
+
+int jb_set_pd_adapter(JbBatch* b, int32_t order, int32_t is_instantaneous, const double* velocity_deadband) {
+    if (!b) return fail(JB_ERR_INVALID_ARGUMENT, "null argument");
+    if (order != 0 && order != 1) return fail(JB_ERR_INVALID_ARGUMENT, "Derivative order of the action out-of-bounds.");
+    if (!b->kp.pdf) return fail(JB_ERR_BAD_CONTROL_FLOW, "the PDController block is not enabled (jb_set_pd_controller_full)");
+    CU(cudaSetDevice(b->device));
+    if (velocity_deadband) {
+        if (!b->d_ad_deadband) { int rc = dev_alloc(b, &b->d_ad_deadband, b->nmotors); if (rc) return rc; }
+        CU(cudaMemcpyAsync(b->d_ad_deadband, velocity_deadband, sizeof(double) * b->nmotors, cudaMemcpyHostToDevice, b->stream));
+        CU(cudaStreamSynchronize(b->stream));
+    }
+    b->ad_order = order; b->ad_instantaneous = is_instantaneous ? 1 : 0; b->ad_has_deadband = velocity_deadband != nullptr;
+    return JB_OK;
+}
+
+int jb_pd_adapter_device(JbBatch* b, const double* action_dev, double step_dt) {
+    if (!b || !action_dev) return fail(JB_ERR_INVALID_ARGUMENT, "null argument");
+    if (!b->kp.pdf) return fail(JB_ERR_BAD_CONTROL_FLOW, "the PDController block is not enabled (jb_set_pd_controller_full)");
+    if (b->ad_order < 0) return fail(JB_ERR_BAD_CONTROL_FLOW, "the PDAdapter block is not configured (jb_set_pd_adapter)");
+    CU(cudaSetDevice(b->device));
+    const size_t total = static_cast<size_t>(b->n_env) * b->nmotors;
+    if (!total) return JB_OK;
+    JB_LAUNCH(pd_adapter_kernel, static_cast<unsigned>((total + 255) / 256), 256, 0, b->stream, action_dev, b->d_pdf_state, b->d_pdf,
+              b->ad_has_deadband ? b->d_ad_deadband : nullptr, b->d_cmd, b->n_env, b->nmotors, b->ad_order, b->ad_instantaneous, step_dt);
+    CU(cudaGetLastError());
+    ++b->launches;
+    return JB_OK;
+}
+
 int jb_set_mahony_filter(JbBatch* b, double kp, double ki) {
     if (!b) return fail(JB_ERR_INVALID_ARGUMENT, "null argument");
     CU(cudaSetDevice(b->device));
@@ -809,17 +892,21 @@ int jb_set_sensor_options(JbBatch* b, int32_t type, int32_t index, const double*
         d.delay = delay; d.jitter = jitter; d.order = delay_interpolation_order;
     }
     b->sp_dirty = true;
+    b->sp_rows_dirty = true;
     return JB_OK;
 }
 
 int jb_set_seeds(JbBatch* b, const uint32_t* seeds) {
     if (!b || !seeds) return fail(JB_ERR_INVALID_ARGUMENT, "null argument");
     b->seeds.assign(seeds, seeds + b->n_env);
+    b->sp_rows_dirty = true;
     return JB_OK;
 }
 
-// Tables, buffers and start states of the pipeline, (re)built at jb_start when options changed
-static int prepare_sensor_pipeline(JbBatch* b, const uint8_t* mask) {
+// Tables, buffers and start states of the pipeline, (re)built at jb_start when options changed.  `rows_if_dirty`
+// (jb_start_device, which has no host mask): the generator start states of ALL envs, and only when the seeds or the
+// sensor set changed since they were last uploaded -- the kernel reads an env's row only when that env (re)starts.
+static int prepare_sensor_pipeline(JbBatch* b, const uint8_t* mask, bool rows_if_dirty = false) {
     if (b->sdesc.empty()) return JB_OK;
     KParams& kp = b->kp;
     const int ns = static_cast<int>(b->sdesc.size());
@@ -882,6 +969,7 @@ static int prepare_sensor_pipeline(JbBatch* b, const uint8_t* mask) {
     // Robot::reset draws one seed per sensor type (robot.cc:137-144; fixed type order Imu, Force, Encoder, Effort, Contact here,
     // the reference iterates an unordered_map), resetAll expands it with a seed_seq into one seed per sensor
     // (abstract_sensor.hxx:213-226) and PCG32(seed) sets state = seed | 3 (random.cc:10-13).
+    if (rows_if_dirty && !b->sp_rows_dirty) return JB_OK;
     if (b->seeds.empty()) b->seeds.assign(b->n_env, 0u);
     std::vector<unsigned long long> init(static_cast<size_t>(b->n_env) * ns, 0ULL);
     const int counts[5] = {kp.nimu, kp.nforce, kp.nenc, kp.neff, kp.ncs};
@@ -911,6 +999,7 @@ static int prepare_sensor_pipeline(JbBatch* b, const uint8_t* mask) {
             if (mask[e]) CU(cudaMemcpyAsync(b->d_sp_rng_init + static_cast<size_t>(e) * ns, init.data() + static_cast<size_t>(e) * ns, sizeof(unsigned long long) * ns, cudaMemcpyHostToDevice, b->stream));
     } else CU(cudaMemcpyAsync(b->d_sp_rng_init, init.data(), sizeof(unsigned long long) * init.size(), cudaMemcpyHostToDevice, b->stream));
     CU(cudaStreamSynchronize(b->stream));
+    if (!mask) b->sp_rows_dirty = false;
     return JB_OK;
 }
 
@@ -963,6 +1052,21 @@ int jb_start(JbBatch* b, const uint8_t* mask, const double* q0, const double* v0
     rc = launch(b, MODE_START, 0.0, mask ? b->d_mask : nullptr);
     if (rc) return rc;
     CU(cudaStreamSynchronize(b->stream));
+    b->any_started = true;
+    return JB_OK;
+}
+
+int jb_start_device(JbBatch* b, const uint8_t* mask_dev, const double* q0_dev, const double* v0_dev) {
+    if (!b || !q0_dev || !v0_dev) return fail(JB_ERR_INVALID_ARGUMENT, "null argument");
+    CU(cudaSetDevice(b->device));
+    CU(cudaMemcpyAsync(b->d_qin, q0_dev, sizeof(double) * b->n_env * b->nq, cudaMemcpyDeviceToDevice, b->stream));
+    CU(cudaMemcpyAsync(b->d_vin, v0_dev, sizeof(double) * b->n_env * b->nv, cudaMemcpyDeviceToDevice, b->stream));
+    if (mask_dev) CU(cudaMemcpyAsync(b->d_mask, mask_dev, b->n_env, cudaMemcpyDeviceToDevice, b->stream));
+    int rc = prepare_sensor_pipeline(b, nullptr, true);
+    if (rc) return rc;
+    // the input checks run in the kernel (LaunchArgs::validate): no decision here depends on device data
+    rc = launch(b, MODE_START, 0.0, mask_dev ? b->d_mask : nullptr, nullptr, true);
+    if (rc) return rc;
     b->any_started = true;
     return JB_OK;
 }
@@ -1305,6 +1409,14 @@ int jb_device_views(JbBatch* b, double** sensors_dev, double** qv_dev) {
     if (!b) return fail(JB_ERR_INVALID_ARGUMENT, "null argument");
     if (sensors_dev) *sensors_dev = b->d_sensors;
     if (qv_dev) *qv_dev = b->d_qv;
+    return JB_OK;
+}
+
+int jb_device_block_views(JbBatch* b, int32_t** status, double** pd_state, double** mahony) {
+    if (!b) return fail(JB_ERR_INVALID_ARGUMENT, "null argument");
+    if (status) *status = b->d_status;
+    if (pd_state) *pd_state = b->kp.pdf ? b->d_pdf_state : nullptr;
+    if (mahony) *mahony = b->kp.mahony ? b->d_mahony : nullptr;
     return JB_OK;
 }
 

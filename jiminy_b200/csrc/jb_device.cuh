@@ -33,7 +33,7 @@ struct LaunchArgs {
     int32_t mode;                  // MODE_*
     int32_t peer_on;               // MODE_STEP of a connected batch: publish the sensor rows to the peers, signal at the end
     int32_t peer_parity;           // which of the two gathered buffers this step fills
-    int32_t pad;
+    int32_t validate;              // MODE_START from device inputs: each env checks its own (q0, v0) row first
     long long peer_step;           // step counter the completion flags are set to
     double step_dt;
     const uint8_t* mask;           // MODE_START: envs to (re)start, null = all
@@ -160,6 +160,8 @@ struct KParams {
     int32_t bd_off, bd_lsh;        // shared-memory region of the sweep (2 x 6 bd_n doubles per env, spread over its lanes); log2(L)
     int32_t bd_rec[4], bd_owner[4], bd_slot[4];   // record of each contact body, owning sub-lane, index among the owner's bodies
     const int32_t* bd_of_contact;  // [ncontacts] contact body of each contact frame
+    // (appended last: the offsets of every field above, which the step path reads, stay what they were)
+    const double* q_bounds;        // [2][nq] position lower / upper bounds, for the input checks of LaunchArgs::validate
 };
 
 // Launch parameters live in constant memory (uniform constant-bank operands in every device

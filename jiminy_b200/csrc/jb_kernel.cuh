@@ -365,6 +365,26 @@ __device__ __forceinline__ void env_step_body(const LaunchArgs& la, const bool o
 
     const bool masked_out = (mode == MODE_START) && la.mask != nullptr && la.mask[c.env] == 0;
     if (masked_out) return;   // whole env (all its lanes) leaves: group masks keep the others safe
+    if constexpr (!FAST) {
+        // jb_start_device: the input checks jb_start runs on the host (Engine::start, engine.cc:1007-1037), per env.  An env
+        // whose row fails them is not started and writes nothing but its status word.
+        if (mode == MODE_START && la.validate) {
+            const double* qe = KP->q_in + static_cast<size_t>(c.env) * KP->nq;
+            const double* ve = KP->v_in + static_cast<size_t>(c.env) * KP->nv;
+            const double* lo = KP->q_bounds;
+            const double* hi = KP->q_bounds + KP->nq;
+            bool bad = false;
+            for (int k = c.sub; k < KP->nq; k += L) {
+                const double x = qe[k];
+                bad = bad || !(x == x) || D_EPS < x - hi[k] || D_EPS < lo[k] - x;
+            }
+            for (int k = c.sub; k < KP->nv; k += L) bad = bad || !(ve[k] == ve[k]);
+            if (jb_any(c, bad)) {
+                if (c.valid && c.sub == 0) KP->status[c.env] = JB_ENV_NOT_STARTED | JB_ENV_BAD_START;
+                return;
+            }
+        }
+    }
     if (mode == MODE_STEP && (status & (JB_ENV_NOT_STARTED | JB_ENV_NAN | JB_ENV_ITER_FAILED | JB_ENV_DT_UNDERFLOW | JB_ENV_SOLVER_FAILED))) {
         JB_EMUL_LEAVES_EARLY(FAST ? 0 : 1);
         return;

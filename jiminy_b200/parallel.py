@@ -60,10 +60,10 @@ def gather_observations(local_obs: torch.Tensor, shard: Shard) -> torch.Tensor:
 
 
 class _DevArray:
-    """Zero-copy torch view of a raw device pointer (CUDA array interface)."""
+    """Zero-copy torch view of a raw device pointer (CUDA array interface); fp64 unless `typestr` says otherwise."""
 
-    def __init__(self, ptr: int, shape):
-        self.__cuda_array_interface__ = {"shape": tuple(shape), "typestr": "<f8", "data": (int(ptr), False), "version": 3}
+    def __init__(self, ptr: int, shape, typestr: str = "<f8"):
+        self.__cuda_array_interface__ = {"shape": tuple(shape), "typestr": typestr, "data": (int(ptr), False), "version": 3}
 
 
 class ObservationExchange:
