@@ -294,6 +294,30 @@ int jb_set_impulse_force(JbBatch* batch, int32_t index, const uint8_t* mask, con
 int jb_register_profile_force(JbBatch* batch, int32_t joint, const double* frame_translation, double update_period,
                               int32_t* slot_out);
 int jb_set_profile_force(JbBatch* batch, int32_t slot, const double* wrench /* [n_env][6] */);
+/* jb_set_impulse_force from device buffers of the same layouts (mask_dev may be NULL: all envs), one small kernel on the
+ * batch stream with no host synchronisation.  Engine::registerImpulseForce's checks (engine.cc:2463-2475) run per env, with
+ * NaN added: a row with a NaN, t < 0 or dt < STEPPER_MIN_TIMESTEP is not written and its env's status becomes
+ * JB_ENV_NOT_STARTED | JB_ENV_BAD_START, as for a row jb_start_device rejects (a later start of that env clears it). */
+int jb_set_impulse_force_device(JbBatch* batch, int32_t index, const uint8_t* mask_dev, const double* t_dev,
+                                const double* dt_dev, const double* wrench_dev);
+/* Replaces: Engine::registerProfileForce(robot, frame, func, 0) where `func` evaluates periodic tabular processes, as the
+ * walker env's disturbance profile does (gym_jiminy locomotion.py:326-330, :340-359, with PeriodicTabularProcess::operator(),
+ * core/src/utilities/random.cc:336-400).  Component component[k] (0..5: linear then angular, world-aligned axes at the
+ * frame origin) of the wrench is the periodic cubic-Hermite table k of each env: n_knots[k] knots evenly spaced over
+ * period[k], evaluated at the env's own time.  update_period == 0: at the time of every dynamics evaluation (every stage
+ * of every stepper, and the evaluations of jb_start at t = 0); update_period > 0: sampled at the multiples of the period
+ * and held, with the breakpoints and the zero-until-the-first-update rule of jb_register_profile_force.  The force has a
+ * slot of its own.  Its tables start at zero; slot_out receives the process-force index. */
+int jb_register_process_force(JbBatch* batch, int32_t joint, const double* frame_translation, double update_period,
+                              int32_t n_comp, const int32_t* component, const int32_t* n_knots, const double* period,
+                              int32_t* slot_out);
+/* Rewrites the tables of process force `slot` for the envs selected by mask (NULL = all): values and grads are
+ * [n_env][sum of n_knots] (knot values and slopes of the tables one after the other; any gain is folded into both by the
+ * caller).  Allowed while envs run; the new tables apply from the next evaluation of those envs.  The _device form takes
+ * device buffers of the same layouts and is enqueued on the batch stream without host synchronisation. */
+int jb_set_process_force(JbBatch* batch, int32_t slot, const uint8_t* mask, const double* values, const double* grads);
+int jb_set_process_force_device(JbBatch* batch, int32_t slot, const uint8_t* mask_dev, const double* values_dev,
+                                const double* grads_dev);
 /* Replaces: Engine::removeAllForces (engine.cc:568-573, :2569-2638). */
 int jb_remove_all_forces(JbBatch* batch);
 

@@ -64,7 +64,9 @@ class Api:
                "jb_get_pd_controller_state", "jb_set_pd_controller_state", "jb_get_constraints",
                "jb_get_stepper_state", "jb_set_stepper_state", "jb_get_centroidal",
                "jb_set_sensor_options", "jb_set_seeds", "jb_get_sensor_data",
-               "jb_start_device", "jb_set_pd_adapter", "jb_pd_adapter_device", "jb_device_block_views")
+               "jb_start_device", "jb_set_pd_adapter", "jb_pd_adapter_device", "jb_device_block_views",
+               "jb_set_impulse_force_device", "jb_register_process_force", "jb_set_process_force",
+               "jb_set_process_force_device")
 
     def __init__(self, cdll: C.CDLL):
         self.dll = L = cdll
@@ -131,6 +133,11 @@ class Api:
         L.jb_set_pd_adapter.argtypes = [vp, C.c_int32, C.c_int32, c_double_p]
         L.jb_pd_adapter_device.argtypes = [vp, vp, C.c_double]
         L.jb_device_block_views.argtypes = [vp, C.POINTER(vp), C.POINTER(vp), C.POINTER(vp)]
+        L.jb_set_impulse_force_device.argtypes = [vp, C.c_int32] + [vp] * 4
+        L.jb_register_process_force.argtypes = [vp, C.c_int32, c_double_p, C.c_double, C.c_int32, c_int32_p, c_int32_p,
+                                                c_double_p, c_int32_p]
+        L.jb_set_process_force.argtypes = [vp, C.c_int32, c_uint8_p, c_double_p, c_double_p]
+        L.jb_set_process_force_device.argtypes = [vp, C.c_int32, vp, vp, vp]
 
     def check(self, rc: int) -> None:
         if rc != JB_OK:
@@ -186,6 +193,7 @@ class BatchedEngine:
         lay = JbSensorLayout()
         self._api.check(self._api.dll.jb_sensor_layout(self._h, C.byref(lay)))
         self.sensor_layout, self.width = lay, lay.width
+        self._process_knots: Dict[int, int] = {}   # knots of each process force (row width of its tables)
 
     def close(self) -> None:
         if getattr(self, "_h", None):
@@ -286,8 +294,50 @@ class BatchedEngine:
         self._api.check(self._api.dll.jb_set_profile_force(self._h, int(slot), dptr(force)))
         self._api.check(self._api.dll.jb_synchronize(self._h))
 
+    def set_impulse_force_device(self, index: int, t_ptr: int, dt_ptr: int, force_ptr: int,
+                                 mask_ptr: Optional[int] = None) -> None:
+        """`set_impulse_force` from device buffers (t, dt [n_env], force [n_env, 6] fp64, mask [n_env] uint8 or None = all),
+        enqueued on the batch stream with no host synchronisation: keep the buffers alive until the stream has passed the
+        call.  A row with a NaN, t < 0 or dt < 1e-10 is not written; its env gets JB_ENV_NOT_STARTED | JB_ENV_BAD_START."""
+        self._api.check(self._api.dll.jb_set_impulse_force_device(self._h, int(index), C.c_void_p(mask_ptr or None),
+                                                                  C.c_void_p(t_ptr), C.c_void_p(dt_ptr), C.c_void_p(force_ptr)))
+
+    def register_process_force(self, frame, components, n_knots, periods, update_period: float = 0.0) -> int:
+        """A force whose wrench component `components[k]` (0..5, world-aligned, at the frame origin) is a periodic
+        cubic-Hermite table of `n_knots[k]` knots over `periods[k]` seconds, per env, evaluated at the env's own time at
+        every dynamics evaluation (update_period 0) or sampled and held at the multiples of `update_period`.  The tables
+        start at zero (`set_process_force`).  Returns the process-force index."""
+        joint, p = self._frame(frame)
+        comp = np.ascontiguousarray(components, dtype=np.int32)
+        nk = np.ascontiguousarray(n_knots, dtype=np.int32)
+        per = np.ascontiguousarray(periods, dtype=np.float64)
+        if not comp.shape == nk.shape == per.shape or comp.ndim != 1:
+            raise ValueError("components, n_knots and periods must be 1-D and of the same length")
+        idx = C.c_int32(-1)
+        self._api.check(self._api.dll.jb_register_process_force(
+            self._h, joint, dptr(p), float(update_period), int(comp.size), comp.ctypes.data_as(c_int32_p),
+            nk.ctypes.data_as(c_int32_p), dptr(per), C.byref(idx)))
+        self._process_knots[int(idx.value)] = int(nk.sum())
+        return int(idx.value)
+
+    def set_process_force(self, index: int, values, grads, mask: Optional[np.ndarray] = None) -> None:
+        """Knot values and slopes [n_env, sum(n_knots)] of process force `index` (tables one after the other) for the envs
+        of `mask` (None = all); the other rows keep their tables."""
+        k = self._process_knots[int(index)]
+        values, grads = self._per_env(values, (k,)), self._per_env(grads, (k,))
+        m = None if mask is None else np.ascontiguousarray(mask, dtype=np.uint8)
+        self._api.check(self._api.dll.jb_set_process_force(self._h, int(index), None if m is None else m.ctypes.data_as(c_uint8_p),
+                                                           dptr(values), dptr(grads)))
+
+    def set_process_force_device(self, index: int, values_ptr: int, grads_ptr: int, mask_ptr: Optional[int] = None) -> None:
+        """`set_process_force` from device buffers (values, grads [n_env, sum(n_knots)] fp64, mask [n_env] uint8 or None),
+        enqueued on the batch stream with no host synchronisation."""
+        self._api.check(self._api.dll.jb_set_process_force_device(self._h, int(index), C.c_void_p(mask_ptr or None),
+                                                                  C.c_void_p(values_ptr), C.c_void_p(grads_ptr)))
+
     def remove_all_forces(self) -> None:
         self._api.check(self._api.dll.jb_remove_all_forces(self._h))
+        self._process_knots.clear()
 
     def set_pd_controller_full(self, kp, kd, state_lower, state_upper, safety=None) -> None:
         """gym_jiminy's `PDController` block on the device (+ `MotorSafetyLimit` when `safety` = [kp, kd, soft_lower,

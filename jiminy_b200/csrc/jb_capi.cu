@@ -5,6 +5,7 @@
 #include <cuda_runtime.h>
 #endif
 
+#include <algorithm>
 #include <cmath>
 #include <cstdio>
 #include <cstring>
@@ -100,11 +101,17 @@ struct JbBatch {
     long long step_id = 0;
     bool peer_enabled = true;                   // jb_peer_obs_enable
     // external forces: frames (slots), impulse table mirror, profile periods
-    struct ExtFrame { int joint; double p[3]; };
+    struct ExtFrame { int joint; double p[3]; bool owned; };   // owned: the slot of a process force, shared with nothing
     std::vector<ExtFrame> eframes;
     std::vector<double> h_imp;      // [MAX_IMPULSE][IMPULSE_ROWS][n_pad]
     ExtSlot* d_eslots = nullptr;
     double *d_imp = nullptr, *d_prof_pending = nullptr, *d_prof_latched = nullptr;
+    bool h_imp_stale = false;       // jb_set_impulse_force_device wrote d_imp behind the host mirror
+    // process forces: tables [2][ktot][n_pad], host-setter staging [2][n_env][ktot], latched values
+    double* d_proc_tab[MAX_PROCESS] = {};
+    double* d_proc_stage[MAX_PROCESS] = {};
+    size_t proc_tab_cap[MAX_PROCESS] = {}, proc_stage_cap[MAX_PROCESS] = {};   // doubles allocated (kept across jb_remove_all_forces)
+    double* d_proc_latched = nullptr;
 };
 
 // The dynamic shared-memory opt-in is a per-function, per-device attribute: only ever raise it.
@@ -139,6 +146,22 @@ static int dev_alloc(JbBatch* b, T** p, size_t count) {
     CU(cudaMemsetAsync(raw, 0, std::max<size_t>(count, 1) * sizeof(T), b->stream));
     b->allocs.push_back(raw);
     *p = static_cast<T*>(raw);
+    return JB_OK;
+}
+
+// A buffer of at least `count` elements in *p (capacity in *cap): reused when large enough, else replaced (the old one is freed)
+template <typename T>
+static int dev_reserve(JbBatch* b, T** p, size_t* cap, size_t count) {
+    if (*p && *cap >= count) return JB_OK;
+    if (*p) {
+        CU(cudaStreamSynchronize(b->stream));
+        b->allocs.erase(std::find(b->allocs.begin(), b->allocs.end(), static_cast<void*>(*p)));
+        CU(cudaFree(*p));
+        *p = nullptr; *cap = 0;
+    }
+    int rc = dev_alloc(b, p, count);
+    if (rc) return rc;
+    *cap = count;
     return JB_OK;
 }
 
@@ -285,6 +308,8 @@ static void apply_options(JbBatch* b, const JbOptions* o) {
     // profile forces with a finite update period add breakpoints (engine.cc:2551-2562)
     for (int j = 0; j < b->kp.n_prof; ++j)
         if (b->kp.prof_period[j] > 2.3e-16) supd = std::min(supd, b->kp.prof_period[j]);
+    for (int j = 0; j < b->kp.n_proc; ++j)
+        if (b->kp.proc_period[j] > 2.3e-16) supd = std::min(supd, b->kp.proc_period[j]);
     b->kp.stepper_update_period = std::isfinite(supd) ? supd : 1e308;
 }
 
@@ -590,6 +615,13 @@ int jb_describe(JbBatch* b, char* buf, int32_t len) {
                   b->kp.fast_bounds ? ", joint bounds solved in the evaluation" : "",
                   !b->kp.cons_on ? "flag only" : (b->kp.cq_on ? (b->kp.lb_on ? "structured quadruped solver + lane-block solver" : "structured quadruped solver + generic")
                                                  : (b->kp.bd_on ? "body-space contact solver + lane-block solver" : (b->kp.lb_on ? "lane-block solver" : "generic solver"))));
+    for (int j = 0; j < b->kp.n_proc; ++j) {
+        const size_t used = std::strlen(buf);
+        if (used + 1 >= static_cast<size_t>(len)) break;
+        std::snprintf(buf + used, len - used, "; process force %d: joint %d, %d periodic tables (%d knots), %s", j,
+                      b->eframes[b->kp.proc_slot[j]].joint, b->kp.proc_ncomp[j], b->kp.proc_ktot[j],
+                      b->kp.proc_period[j] > 2.3e-16 ? "sampled at its update period" : "evaluated at every dynamics evaluation");
+    }
     return JB_OK;
 }
 
@@ -1082,11 +1114,13 @@ int jb_stop(JbBatch* b) {
     return JB_OK;
 }
 
-static int ext_slot_for(JbBatch* b, int joint, const double* p, int* slot_out) {
+// `own`: a slot of its own, which no later force shares (a process force writes its slot's wrench before every evaluation,
+// so whatever else the slot held would be lost); other forces share the slot of their frame
+static int ext_slot_for(JbBatch* b, int joint, const double* p, int* slot_out, bool own = false) {
     if (joint <= 0 || joint >= b->njoints) return fail(JB_ERR_INVALID_ARGUMENT, "Impossible to apply external forces to the universe itself (or unknown joint).");
-    for (size_t e = 0; e < b->eframes.size(); ++e) {
+    for (size_t e = 0; e < b->eframes.size() && !own; ++e) {
         const auto& f = b->eframes[e];
-        if (f.joint == joint && f.p[0] == p[0] && f.p[1] == p[1] && f.p[2] == p[2]) { *slot_out = static_cast<int>(e); return JB_OK; }
+        if (!f.owned && f.joint == joint && f.p[0] == p[0] && f.p[1] == p[1] && f.p[2] == p[2]) { *slot_out = static_cast<int>(e); return JB_OK; }
     }
     if (b->eframes.size() >= MAX_ESLOT) return fail(JB_ERR_NOT_IMPLEMENTED, "too many distinct frames carrying external forces");
     const Plan& P = b->plan;
@@ -1101,11 +1135,12 @@ static int ext_slot_for(JbBatch* b, int joint, const double* p, int* slot_out) {
         b->kp.eslots = b->d_eslots; b->kp.imp_data = b->d_imp;
         b->kp.prof_pending = b->d_prof_pending; b->kp.prof_latched = b->d_prof_latched;
     }
-    const size_t smem = static_cast<size_t>(b->base_fields + ESLOT_SIZE * (b->eframes.size() + 1)) * 32 * sizeof(double);
+    // + 1 field behind the slots: the time of the step being taken (stage times of the process forces)
+    const size_t smem = static_cast<size_t>(b->base_fields + ESLOT_SIZE * (b->eframes.size() + 1) + 1) * 32 * sizeof(double);
     if (smem > 227 * 1024) return fail(JB_ERR_NOT_IMPLEMENTED, "no shared memory left for an external-force slot");
     int rc = raise_smem_attr(b->device, smem);
     if (rc) return rc;
-    JbBatch::ExtFrame f{joint, {p[0], p[1], p[2]}};
+    JbBatch::ExtFrame f{joint, {p[0], p[1], p[2]}, own};
     b->eframes.push_back(f);
     std::vector<ExtSlot> rows(b->eframes.size() * P.L);
     for (size_t e = 0; e < b->eframes.size(); ++e)
@@ -1128,6 +1163,11 @@ static int ext_slot_for(JbBatch* b, int joint, const double* p, int* slot_out) {
 
 static int upload_impulse(JbBatch* b, int k, const uint8_t* mask, const double* t, const double* dt, const double* wrench) {
     const size_t N = b->n_pad;
+    if (b->h_imp_stale) {
+        CU(cudaMemcpyAsync(b->h_imp.data(), b->d_imp, sizeof(double) * b->h_imp.size(), cudaMemcpyDeviceToHost, b->stream));
+        CU(cudaStreamSynchronize(b->stream));
+        b->h_imp_stale = false;
+    }
     double* rows = b->h_imp.data() + static_cast<size_t>(k) * IMPULSE_ROWS * N;
     for (int i = 0; i < b->n_env; ++i) {
         if (mask && !mask[i]) continue;
@@ -1167,10 +1207,8 @@ int jb_set_impulse_force(JbBatch* b, int32_t index, const uint8_t* mask, const d
     return upload_impulse(b, index, mask, t, dt, wrench);
 }
 
-int jb_register_profile_force(JbBatch* b, int32_t joint, const double* frame_translation, double update_period, int32_t* slot_out) {
-    if (!b || !frame_translation) return fail(JB_ERR_INVALID_ARGUMENT, "null argument");
-    if (b->any_started) return fail(JB_ERR_BAD_CONTROL_FLOW, "Simulation already running. Please stop it before registering new forces.");
-    if (b->kp.n_prof >= MAX_PROFILE) return fail(JB_ERR_NOT_IMPLEMENTED, "too many profile forces");
+// Engine::registerProfileForce's checks of the update period (engine.cc:2527-2548)
+static int check_profile_period(JbBatch* b, double update_period) {
     if (update_period > 2.3e-16 && update_period < 1e-6)
         return fail(JB_ERR_INVALID_ARGUMENT, "Cannot register external force profile with update period smaller than 1e-06s.");
     if (update_period > 2.3e-16 && b->kp.stepper_update_period < 1e300) {
@@ -1179,6 +1217,14 @@ int jb_register_profile_force(JbBatch* b, int32_t joint, const double* frame_tra
         if (std::min(r, lo - r) > 1e-12)
             return fail(JB_ERR_INVALID_ARGUMENT, "In discrete mode, the update period of force profiles and the stepper update period must be multiple of each other.");
     }
+    return JB_OK;
+}
+
+int jb_register_profile_force(JbBatch* b, int32_t joint, const double* frame_translation, double update_period, int32_t* slot_out) {
+    if (!b || !frame_translation) return fail(JB_ERR_INVALID_ARGUMENT, "null argument");
+    if (b->any_started) return fail(JB_ERR_BAD_CONTROL_FLOW, "Simulation already running. Please stop it before registering new forces.");
+    if (b->kp.n_prof >= MAX_PROFILE) return fail(JB_ERR_NOT_IMPLEMENTED, "too many profile forces");
+    if (int rc0 = check_profile_period(b, update_period)) return rc0;
     CU(cudaSetDevice(b->device));
     int slot = 0;
     int rc = ext_slot_for(b, joint, frame_translation, &slot);
@@ -1211,10 +1257,138 @@ int jb_set_profile_force(JbBatch* b, int32_t slot, const double* wrench) {
     return JB_OK;
 }
 
+// Masked rewrite of impulse `index` from device rows, one thread per padded env (padding envs follow the last env, like
+// upload_impulse).  A row that fails Engine::registerImpulseForce's checks is not written; its env is flagged like a
+// failed jb_start_device.
+__global__ void set_impulse_kernel(double* __restrict__ rows, int32_t* __restrict__ status, const uint8_t* __restrict__ mask,
+                                   const double* __restrict__ t, const double* __restrict__ dt, const double* __restrict__ wrench,
+                                   int n_env, int n_pad) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n_pad) return;
+    const int src = i < n_env ? i : n_env - 1;
+    if (mask && !mask[src]) return;
+    const double ti = t[src], dti = dt[src];
+    bool bad = !(ti == ti) || !(dti == dti) || ti < 0.0 || dti < STEPPER_MIN_TIMESTEP;
+    for (int c = 0; c < 6; ++c) bad = bad || !(wrench[static_cast<size_t>(src) * 6 + c] == wrench[static_cast<size_t>(src) * 6 + c]);
+    if (bad) {
+        if (i < n_env) status[i] = JB_ENV_NOT_STARTED | JB_ENV_BAD_START;
+        return;
+    }
+    rows[i] = ti; rows[n_pad + i] = dti;
+    if (i < n_env)
+        for (int c = 0; c < 6; ++c) rows[static_cast<size_t>(2 + c) * n_pad + i] = wrench[static_cast<size_t>(i) * 6 + c];
+}
+
+int jb_set_impulse_force_device(JbBatch* b, int32_t index, const uint8_t* mask_dev, const double* t_dev, const double* dt_dev,
+                                const double* wrench_dev) {
+    if (!b || !t_dev || !dt_dev || !wrench_dev) return fail(JB_ERR_INVALID_ARGUMENT, "null argument");
+    if (index < 0 || index >= b->kp.n_imp) return fail(JB_ERR_INVALID_ARGUMENT, "unknown impulse force");
+    CU(cudaSetDevice(b->device));
+    JB_LAUNCH(set_impulse_kernel, static_cast<unsigned>((b->n_pad + 127) / 128), 128, 0, b->stream,
+              b->d_imp + static_cast<size_t>(index) * IMPULSE_ROWS * b->n_pad, b->d_status, mask_dev, t_dev, dt_dev, wrench_dev,
+              b->n_env, b->n_pad);
+    CU(cudaGetLastError());
+    ++b->launches;
+    b->h_imp_stale = true;
+    return JB_OK;
+}
+
+int jb_register_process_force(JbBatch* b, int32_t joint, const double* frame_translation, double update_period, int32_t n_comp,
+                              const int32_t* component, const int32_t* n_knots, const double* period, int32_t* slot_out) {
+    if (!b || !frame_translation || !component || !n_knots || !period) return fail(JB_ERR_INVALID_ARGUMENT, "null argument");
+    if (b->any_started) return fail(JB_ERR_BAD_CONTROL_FLOW, "Simulation already running. Please stop it before registering new forces.");
+    if (b->kp.n_proc >= MAX_PROCESS) return fail(JB_ERR_NOT_IMPLEMENTED, "too many process forces");
+    if (n_comp < 1 || n_comp > 6) return fail(JB_ERR_INVALID_ARGUMENT, "a process force has 1 to 6 tables");
+    int ktot = 0;
+    for (int k = 0; k < n_comp; ++k) {
+        if (component[k] < 0 || component[k] > 5) return fail(JB_ERR_INVALID_ARGUMENT, "wrench component out of range [0, 5]");
+        for (int m = 0; m < k; ++m)
+            if (component[m] == component[k]) return fail(JB_ERR_INVALID_ARGUMENT, "wrench component given twice");
+        if (n_knots[k] < 1) return fail(JB_ERR_INVALID_ARGUMENT, "a table needs at least one knot");
+        if (!(period[k] > 0.0) || !std::isfinite(period[k])) return fail(JB_ERR_INVALID_ARGUMENT, "table period must be positive and finite");
+        ktot += n_knots[k];
+    }
+    if (int rc0 = check_profile_period(b, update_period)) return rc0;
+    CU(cudaSetDevice(b->device));
+    int slot = 0;
+    int rc = ext_slot_for(b, joint, frame_translation, &slot, true);
+    if (rc) return rc;
+    const int j = b->kp.n_proc;
+    const size_t N = b->n_pad;
+    if (!b->d_proc_latched && (rc = dev_alloc(b, &b->d_proc_latched, static_cast<size_t>(MAX_PROCESS) * 6 * N))) return rc;
+    if ((rc = dev_reserve(b, &b->d_proc_tab[j], &b->proc_tab_cap[j], 2 * static_cast<size_t>(ktot) * N))) return rc;
+    if ((rc = dev_reserve(b, &b->d_proc_stage[j], &b->proc_stage_cap[j], 2 * static_cast<size_t>(ktot) * b->n_env))) return rc;
+    CU(cudaMemsetAsync(b->d_proc_tab[j], 0, sizeof(double) * 2 * ktot * N, b->stream));
+    KParams& kp = b->kp;
+    kp.proc_slot[j] = slot;
+    kp.proc_period[j] = update_period;
+    kp.proc_ncomp[j] = n_comp;
+    kp.proc_ktot[j] = ktot;
+    for (int k = 0, off = 0; k < n_comp; off += n_knots[k], ++k) {
+        kp.proc_comp[j][k] = component[k];
+        kp.proc_nknots[j][k] = n_knots[k];
+        kp.proc_koff[j][k] = off;
+        kp.proc_tperiod[j][k] = period[k];
+        kp.proc_delta[j][k] = period[k] / static_cast<double>(n_knots[k]);   // PeriodicTabularProcess::dt_
+    }
+    kp.proc_tab[j] = b->d_proc_tab[j];
+    kp.proc_latched = b->d_proc_latched;
+    CU(cudaMemsetAsync(b->d_proc_latched + static_cast<size_t>(j) * 6 * N, 0, sizeof(double) * 6 * N, b->stream));
+    kp.n_proc = j + 1;
+    const JbOptions o = kp.opt;
+    apply_options(b, &o);
+    CU(cudaStreamSynchronize(b->stream));
+    if (slot_out) *slot_out = j;
+    return JB_OK;
+}
+
+// Masked rewrite of the tables of one process force, one thread per (knot, padded env); rows [n_env][ktot] in.
+__global__ void set_process_kernel(double* __restrict__ tab, const uint8_t* __restrict__ mask, const double* __restrict__ values,
+                                   const double* __restrict__ grads, int n_env, int n_pad, int ktot) {
+    const size_t idx = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x;
+    if (idx >= static_cast<size_t>(ktot) * n_pad) return;
+    const int k = static_cast<int>(idx / n_pad), i = static_cast<int>(idx % n_pad);
+    const int src = i < n_env ? i : n_env - 1;
+    if (mask && !mask[src]) return;
+    tab[idx] = values[static_cast<size_t>(src) * ktot + k];
+    tab[static_cast<size_t>(ktot) * n_pad + idx] = grads[static_cast<size_t>(src) * ktot + k];
+}
+
+static int launch_set_process(JbBatch* b, int j, const uint8_t* mask, const double* values, const double* grads) {
+    const size_t total = static_cast<size_t>(b->kp.proc_ktot[j]) * b->n_pad;
+    JB_LAUNCH(set_process_kernel, static_cast<unsigned>((total + 255) / 256), 256, 0, b->stream, b->d_proc_tab[j], mask, values,
+              grads, b->n_env, b->n_pad, b->kp.proc_ktot[j]);
+    CU(cudaGetLastError());
+    ++b->launches;
+    return JB_OK;
+}
+
+int jb_set_process_force(JbBatch* b, int32_t slot, const uint8_t* mask, const double* values, const double* grads) {
+    if (!b || !values || !grads) return fail(JB_ERR_INVALID_ARGUMENT, "null argument");
+    if (slot < 0 || slot >= b->kp.n_proc) return fail(JB_ERR_INVALID_ARGUMENT, "unknown process force");
+    CU(cudaSetDevice(b->device));
+    const size_t rows = static_cast<size_t>(b->n_env) * b->kp.proc_ktot[slot];
+    double* st = b->d_proc_stage[slot];
+    CU(cudaMemcpyAsync(st, values, sizeof(double) * rows, cudaMemcpyHostToDevice, b->stream));
+    CU(cudaMemcpyAsync(st + rows, grads, sizeof(double) * rows, cudaMemcpyHostToDevice, b->stream));
+    if (mask) CU(cudaMemcpyAsync(b->d_mask, mask, b->n_env, cudaMemcpyHostToDevice, b->stream));
+    int rc = launch_set_process(b, slot, mask ? b->d_mask : nullptr, st, st + rows);
+    if (rc) return rc;
+    CU(cudaStreamSynchronize(b->stream));
+    return JB_OK;
+}
+
+int jb_set_process_force_device(JbBatch* b, int32_t slot, const uint8_t* mask_dev, const double* values_dev, const double* grads_dev) {
+    if (!b || !values_dev || !grads_dev) return fail(JB_ERR_INVALID_ARGUMENT, "null argument");
+    if (slot < 0 || slot >= b->kp.n_proc) return fail(JB_ERR_INVALID_ARGUMENT, "unknown process force");
+    CU(cudaSetDevice(b->device));
+    return launch_set_process(b, slot, mask_dev, values_dev, grads_dev);
+}
+
 int jb_remove_all_forces(JbBatch* b) {
     if (!b) return fail(JB_ERR_INVALID_ARGUMENT, "null argument");
     if (b->any_started) return fail(JB_ERR_BAD_CONTROL_FLOW, "Simulation already running. Please stop it before removing forces.");
-    b->kp.n_imp = 0; b->kp.n_prof = 0; b->kp.n_eslot = 0;
+    b->kp.n_imp = 0; b->kp.n_prof = 0; b->kp.n_eslot = 0; b->kp.n_proc = 0;
     b->eframes.clear();
     b->smem_bytes = static_cast<size_t>(b->base_fields) * 32 * sizeof(double);
     const JbOptions o = b->kp.opt;

@@ -162,6 +162,20 @@ struct KParams {
     const int32_t* bd_of_contact;  // [ncontacts] contact body of each contact frame
     // (appended last: the offsets of every field above, which the step path reads, stay what they were)
     const double* q_bounds;        // [2][nq] position lower / upper bounds, for the input checks of LaunchArgs::validate
+    // process forces (jb_register_process_force): wrench component proc_comp[j][k] of force j is the periodic cubic-Hermite
+    // table k, values | grads of each env in proc_tab[j] = [2][proc_ktot[j]][n_pad], table k from knot proc_koff[j][k]
+    int32_t n_proc;
+    int32_t proc_slot[MAX_PROCESS];
+    int32_t proc_ncomp[MAX_PROCESS];
+    int32_t proc_ktot[MAX_PROCESS];
+    int32_t proc_comp[MAX_PROCESS][6];
+    int32_t proc_nknots[MAX_PROCESS][6];
+    int32_t proc_koff[MAX_PROCESS][6];
+    double proc_tperiod[MAX_PROCESS][6];   // table period
+    double proc_delta[MAX_PROCESS][6];     // knot spacing period / n_knots
+    double proc_period[MAX_PROCESS];       // update period: 0 = at every dynamics evaluation
+    const double* proc_tab[MAX_PROCESS];
+    double* proc_latched;                  // [MAX_PROCESS][6][n_pad]: value held since the last update (finite period)
 };
 
 // Launch parameters live in constant memory (uniform constant-bank operands in every device
@@ -1860,6 +1874,61 @@ __device__ __noinline__ void stage_quadruped_crba(const Ctx c, const double wq, 
     if (quadruped_crba<true>(c, false, status, wq, kv1, ka1, kvf, kaf, wb)) *status |= ENV_RETRY_FULL;
 }
 
+// ------------------------------------------------------------------------------------------
+// Process forces: the wrench of force j at time t, each component a periodic table of knot values and slopes of this env
+// (PeriodicTabularProcess::operator(), core/src/utilities/random.cc:336-400: t wrapped into [0, P) with a negative
+// remainder shifted by P, left knot floor(t / delta), right knot modulo n, cubicInterp).  The wrap is t - P floor(t / P):
+// fmod's result up to rounding (exact for P = 1 s), and a wrapped time that rounds to P itself takes the last interval
+// at ratio 1, which is the value of knot 0.  (A call to the library's fmod here perturbs the code ptxas gives the hot path.)
+// ------------------------------------------------------------------------------------------
+JB_DI void process_wrench(const Ctx& c, int j, double t, double* F) {
+    const size_t N = KP->n_pad, col = c.env;
+    const int K = KP->proc_ktot[j];
+#pragma unroll
+    for (int k = 0; k < 6; ++k) F[k] = 0.0;
+    for (int k = 0; k < KP->proc_ncomp[j]; ++k) {
+        const int n = KP->proc_nknots[j][k];
+        const double P = KP->proc_tperiod[j][k], delta = KP->proc_delta[j][k];
+        const double x = t - P * floor(t / P);
+        const double quot = x / delta;
+        int il = static_cast<int>(floor(quot));
+        il = il < 0 ? 0 : (il > n - 1 ? n - 1 : il);
+        const int ir = il + 1 == n ? 0 : il + 1;
+        const double ratio = quot - static_cast<double>(il);
+        const double* vals = KP->proc_tab[j] + static_cast<size_t>(KP->proc_koff[j][k]) * N + col;
+        const double* grads = vals + static_cast<size_t>(K) * N;
+        const double yl = vals[il * N], yr = vals[ir * N];
+        const double dy = yr - yl;
+        const double a = grads[il * N] * delta - dy;
+        const double b = -grads[ir * N] * delta + dy;
+        F[KP->proc_comp[j][k]] += yl + ratio * ((1.0 - ratio) * ((1.0 - ratio) * a + ratio * b) + dy);
+    }
+}
+// per-lane shared-memory field behind the external-force slots: time of the accepted state of the step being taken
+JB_DI int proc_time_field() { return KP->ext_off + ESLOT_SIZE * KP->n_eslot; }
+// Process forces with update period 0 at the time `t` of the coming dynamics evaluation (every stage of every stepper,
+// Engine::computeExternalForces called from computeRobotsDynamics, engine.cc:3455-3495): the slot of the force holds the
+// wrench the sweeps apply.
+__device__ __noinline__ void eval_process_forces(const Ctx c, double t) {
+    for (int j = 0; j < KP->n_proc; ++j) {
+        if (KP->proc_period[j] > D_EPS) continue;
+        double F[6];
+        process_wrench(c, j, t, F);
+        double* const xp = jb_smem + (KP->ext_off + ESLOT_SIZE * KP->proc_slot[j]) * 32 + c.lane;
+#pragma unroll
+        for (int k = 0; k < 6; ++k) xp[k * 32] = F[k];
+    }
+}
+// The same at a stage of a step, `t + w` (w = c_i dt of the tableau).  Only the steppers of SigDynamicProc, the signature
+// of batches with process forces, carry it: the instances every other batch runs stay as they were.
+struct SigDynamicProc : SigDynamic<false> {};
+template <class SIG> struct sig_has_proc { static constexpr bool value = false; };
+template <> struct sig_has_proc<SigDynamicProc> { static constexpr bool value = true; };
+template <class SIG>
+JB_DI void eval_process_stage(const Ctx& c, double w) {
+    if constexpr (sig_has_proc<SIG>::value) eval_process_forces(c, SMF(c, proc_time_field()) + w);
+}
+
 // Engine::computeRobotsDynamics: the sweeps give the unconstrained accelerations; then the constraint path
 // (Engine::computeAcceleration with enabled constraints, engine.cc:3709-3866) corrects them if needed.
 // Joint position bounds (computePositionLimitsForcesAlgo, engine.cc:3253-3338): leaving [lo, hi] enables the
@@ -2085,6 +2154,7 @@ template <class SIG>
 __device__ __noinline__ void step_euler_t(const Ctx c, double dt, int* status) {
     // x <- x (+) dt * dx ; dx <- f(t + dt, x)
     make_stage<SIG>(c, dt, R1_V, R1_A, RF_V, RF_A);
+    eval_process_stage<SIG>(c, dt);
     rhs_sig<SIG>(c, false, status);
     SIG::for_each_forward([&](auto r_) {
         const int r = r_;
@@ -2139,6 +2209,7 @@ __device__ __noinline__ void step_rk4_t(const Ctx c, double dt, int* status) {
         }
         if (i == 1) make_stage<SIG>(c, w, R1_V, R1_A, RF_V, RF_A);
         else make_stage<SIG>(c, w, R1_VS, R1_A, RF_VS, RF_A);
+        eval_process_stage<SIG>(c, w);
         rhs_sig<SIG>(c, false, status);
         const double wb = dt * (i == 3 ? 1.0 / 6.0 : 1.0 / 3.0);
         SIG::for_each_forward([&](auto r_) {
@@ -2179,6 +2250,7 @@ __device__ __noinline__ void step_rk4_t(const Ctx c, double dt, int* status) {
             RP(R1_V) = RP(R1_VS);
         }
     });
+    eval_process_stage<SIG>(c, dt);
     if (!one_call) rhs_sig<SIG>(c, false, status);
 }
 
@@ -2198,6 +2270,7 @@ JB_DI void step_euler(const Ctx c, double dt, int* status) {
         else step_euler_t<FastOf<SigDynamic<false>>>(c, dt, status);
     } else {
         if (KP->sig_id == SigQuadruped::ID) step_euler_t<SigQuadruped>(c, dt, status);
+        else if (KP->n_proc > 0) step_euler_t<SigDynamicProc>(c, dt, status);
         else step_euler_t<SigDynamic<false>>(c, dt, status);
     }
 }
@@ -2208,6 +2281,7 @@ JB_DI void step_rk4(const Ctx c, double dt, int* status) {
         else step_rk4_t<FastOf<SigDynamic<false>>>(c, dt, status);
     } else {
         if (KP->sig_id == SigQuadruped::ID) step_rk4_t<SigQuadruped>(c, dt, status);
+        else if (KP->n_proc > 0) step_rk4_t<SigDynamicProc>(c, dt, status);
         else step_rk4_t<SigDynamic<false>>(c, dt, status);
     }
 }
@@ -2340,6 +2414,7 @@ __device__ __noinline__ int step_dopri(const Ctx c, double* dt_io, int* status) 
                 RP(R1_VS) = vs;
             }
         }
+        if (KP->n_proc > 0) eval_process_forces(c, SMF(c, proc_time_field()) + dopri::Cn[i] * h);
         rhs(c, false, status);
         for (int r = 0; r < KP->nrec; ++r) {
             const RecInt* ri = KP->rint + (r * L + c.sub);
@@ -2517,6 +2592,24 @@ JB_DI double refresh_external_forces(const Ctx& c, double t, bool at_start, bool
             for (int k = 0; k < 6; ++k) F[k] = pend[k * N];
         }
         double* const xp = jb_smem + (KP->ext_off + ESLOT_SIZE * KP->prof_slot[j]) * 32 + c.lane;
+#pragma unroll
+        for (int k = 0; k < 6; ++k) xp[k * 32] += F[k];
+    }
+    // process forces with a finite update period: sampled at the updates like the profile forces above (those with period 0
+    // are written before every dynamics evaluation, eval_process_forces)
+    for (int j = 0; j < KP->n_proc; ++j) {
+        const double P = KP->proc_period[j];
+        if (!(P > D_EPS)) continue;
+        double* lat = KP->proc_latched + static_cast<size_t>(j) * 6 * N + col;
+        const bool hit = !at_start && finite_period && period_hit(t, P);
+        double F[6];
+        if (hit) { changed = true; process_wrench(c, j, t, F); }
+#pragma unroll
+        for (int k = 0; k < 6; ++k) {
+            F[k] = at_start ? 0.0 : (hit ? F[k] : lat[k * N]);
+            if ((hit || at_start) && c.valid && c.sub == 0) lat[k * N] = F[k];
+        }
+        double* const xp = jb_smem + (KP->ext_off + ESLOT_SIZE * KP->proc_slot[j]) * 32 + c.lane;
 #pragma unroll
         for (int k = 0; k < 6; ++k) xp[k * 32] += F[k];
     }

@@ -458,6 +458,7 @@ __device__ __forceinline__ void env_step_body(const LaunchArgs& la, const bool o
         iter = 0; iterFailed = 0;
         if (KP->pd_gains != nullptr || KP->pdf != nullptr) update_pd_commands(c, false);
         if (KP->n_eslot > 0) { bool ch = false; refresh_external_forces(c, 0.0, true, false, ch); }
+        if (KP->n_proc > 0) eval_process_forces(c, 0.0);
         stage_from_accepted(c);
         if (KP->cons_on) {
             // resetConstraints, then the INIT_ITERATIONS fixed point of engine.cc:1400-1467: the first evaluation sees
@@ -520,7 +521,10 @@ __device__ __forceinline__ void env_step_body(const LaunchArgs& la, const bool o
             int rc = 0;
             // successive constraint-solver failures are rolled back with a failed step (engine.cc:2104-2112, :2211-2217)
             double solveFailedBackup = 0.0;
-            if constexpr (!FAST) { if (KP->cons_on) solveFailedBackup = CST(CS_SOLVE_FAILED); }
+            if constexpr (!FAST) {
+                if (KP->cons_on) solveFailedBackup = CST(CS_SOLVE_FAILED);
+                if (KP->n_proc > 0) SMF(c, proc_time_field()) = t;   // stage times of the process forces
+            }
             if (opt.ode_solver == JB_SOLVER_EULER_EXPLICIT) { step_euler<FAST>(c, dtLargest, &status); dtLargest = D_INF; }
             else if (FAST || opt.ode_solver == JB_SOLVER_RUNGE_KUTTA_4) { step_rk4<FAST>(c, dtLargest, &status); dtLargest = D_INF; }
             else { if constexpr (!FAST) rc = step_dopri(c, &dtLargest, &status); }
@@ -577,6 +581,7 @@ __device__ __forceinline__ void env_step_body(const LaunchArgs& la, const bool o
             }
             if (!finitePeriod && hasDynamicsChanged) {
                 stage_from_accepted(c);
+                if constexpr (!FAST) { if (KP->n_proc > 0) eval_process_forces(c, t); }
                 if constexpr (FAST) rhs_fast(c, !need_refresh, &status); else rhs(c, !need_refresh, &status);
                 need_refresh = false;
                 hasDynamicsChanged = false;
@@ -592,6 +597,7 @@ __device__ __forceinline__ void env_step_body(const LaunchArgs& la, const bool o
                     if (hasDynamicsChanged) {
                         // FSAL repair: same state, cached contact forces, new command (engine.cc:2032-2037)
                         stage_from_accepted(c);
+                        if constexpr (!FAST) { if (KP->n_proc > 0) eval_process_forces(c, t); }
                         if constexpr (FAST) rhs_fast(c, !need_refresh, &status); else rhs(c, !need_refresh, &status);
                         need_refresh = false;
                         hasDynamicsChanged = false;

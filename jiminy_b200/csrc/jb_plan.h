@@ -111,6 +111,7 @@ constexpr int CS_JOINT_SIZE = 4;
 constexpr int CS_CONTACT_SIZE = 17;      // per contact constraint: enabled, lambda[4], reference R[9], p[3]
 
 constexpr int MAX_ESLOT = 4, MAX_IMPULSE = 16, MAX_PROFILE = 4;
+constexpr int MAX_PROCESS = 2;   // process forces (jb_register_process_force), each on a slot of its own
 constexpr int ESLOT_SIZE = 12;   // wrench in world-aligned axes at the frame origin (6) | same wrench in the joint frame (6)
 constexpr int IMPULSE_ROWS = 8;  // t, dt, wrench[6]
 

@@ -22,6 +22,7 @@ from typing import Any, Dict, Optional, Tuple
 import numpy as np
 
 from . import core, scenarios
+from .disturbance import from_std_ratio
 from .model import RobotTable
 
 SENSOR_FIELDS = {"ImuSensor": 6, "ForceSensor": 6, "EncoderSensor": 2, "EffortSensor": 1, "ContactSensor": 3}
@@ -101,7 +102,9 @@ def configure_pd_blocks(env, kp, kd, joint_position_margin: float, joint_velocit
 
 class BatchedJiminyEnv:
     def __init__(self, scenario: scenarios.Scenario, device: int = 0, height_threshold_ratio: float = 0.5,
-                 simulation_duration_max: float = 20.0, api_: Optional[core.Api] = None):
+                 simulation_duration_max: float = 20.0, api_: Optional[core.Api] = None, std_ratio: Optional[dict] = None):
+        """`std_ratio`: the reference walker env's randomisation ratios.  None or {}: none; {"disturbance": r}: the walker
+        disturbance forces (`jiminy_b200.disturbance`), re-drawn for every env that (re)starts."""
         self.sc = scenario
         self.robot: RobotTable = scenario.robot
         self.n_env, self.step_dt = scenario.n_env, scenario.step_dt
@@ -121,6 +124,10 @@ class BatchedJiminyEnv:
         else:
             iq = np.array([self.robot.idx_q[m.joint] for m in self.robot.motors])
             self.action_low, self.action_high = self.robot.q_lower[iq], self.robot.q_upper[iq]
+        self.disturbance = from_std_ratio(self.robot, std_ratio, simulation_duration_max)
+        if self.disturbance is not None:
+            self.disturbance.register(self.engine)
+            self._disturbance_rng = np.random.default_rng([scenario.seed, 0xD157])
         self._started = False
 
     # ------------------------------------------------------------------ helpers
@@ -140,16 +147,24 @@ class BatchedJiminyEnv:
         sc = scenarios.make(self.sc.name, n, seed=int(self._rng.integers(0, 2 ** 31 - 1)))
         return sc.q0, sc.v0
 
+    def _redraw_disturbance(self, mask: Optional[np.ndarray]) -> None:
+        """New disturbance rows for the envs about to (re)start (`_setup` runs at every reset, locomotion.py:298-330)."""
+        if self.disturbance is not None:
+            draw = self.disturbance.draw_numpy(self._disturbance_rng, self.n_env)
+            self.disturbance.apply_host(self.engine, draw, mask)
+
     # ------------------------------------------------------------------ gym API
     def reset(self, mask: Optional[np.ndarray] = None) -> Tuple[Dict[str, Any], Dict[str, Any]]:
         if mask is None or not self._started:
             q0, v0 = (self.sc.q0, self.sc.v0) if not self._started else self._sample_state(self.n_env)
             self.engine.set_command(self.sc.target0)
+            self._redraw_disturbance(None)
             self.engine.start(q0, v0)
             self.num_steps[:] = 0
             self._started = True
         elif mask.any():
             q0, v0 = self._sample_state(self.n_env)
+            self._redraw_disturbance(mask)
             self.engine.start(q0, v0, mask=mask)
             self.num_steps[mask.astype(bool)] = 0
         return self._observation(), {}
@@ -216,6 +231,7 @@ class PDControlBatchedEnv(BatchedJiminyEnv):
             # no simulation running: the adapter's dt is 0, the target accelerations stay 0 (:652-662)
             self.engine.set_command(np.zeros((self.n_env, self.robot.nmotors)))
             q0, v0 = (self.sc.q0, self.sc.v0) if not self._started else self._sample_state(self.n_env)
+            self._redraw_disturbance(None)
             self.engine.start(q0, v0)
             self.num_steps[:] = 0
             self._started = True

@@ -18,6 +18,14 @@ restart rows are drawn on the device, with replacement, from a fixed bank `reset
 default bank is one such sample of `n_env` rows.  The bank is validated once on the host.  `info["reset_rows"]` gives the
 bank row each env restarted from (-1: not restarted).  This is the one semantic difference from the host env.
 
+Disturbance.  With `std_ratio={"disturbance": r}` the walker disturbance (`jiminy_b200.disturbance`) of the envs in the
+done mask is re-drawn with a torch generator on the device and written by the device setters before the masked restart,
+at every step.  `env.disturbance_rows` holds the impulse schedule and process tables every env currently runs with
+(device tensors, `WalkerDisturbance.draw_torch` layout), so that a run can be replayed through the host setters.  The
+impulse setter's checks (NaN, t < 0, dt < 1e-10) flag a rejected row's env NOT_STARTED | BAD_START, but the masked restart
+enqueued right after it clears that flag and the env runs on with its previous impulse row: the sampler never draws such a
+row (t >= 1.75 s, dt = 10 ms, finite wrenches), so nothing here depends on the flag.
+
 Streams.  All work runs on the batch's own stream (`torch.cuda.ExternalStream(engine.stream())`).  On entry it waits
 for the caller's current stream; on exit the caller's current stream waits for it.  With the CPU emulation of the
 library (`api_` given), device memory is host memory: the env then runs on `torch_device="cpu"`, without streams.
@@ -86,6 +94,12 @@ class DeviceBatchedEnv(envs.BatchedJiminyEnv):
         self._action = torch.zeros((n, nm), **f64)
         self._q_start, self._v_start = torch.zeros((n, self.robot.nq), **f64), torch.zeros((n, self.robot.nv), **f64)
         self._mask = torch.zeros(n, dtype=torch.uint8, device=dev)
+        if self.disturbance is not None:
+            # the tables and schedule every env currently runs with, drawn on the device (`env.disturbance_rows`)
+            self._disturbance_gen = torch.Generator(device=dev)
+            self._disturbance_gen.manual_seed(int(np.random.default_rng([self.sc.seed, 0xD157]).integers(0, 2 ** 31 - 1)))
+            with self._on_batch_stream():     # the draw's first use of its kernels on the batch stream happens here
+                self.disturbance_rows = self.disturbance.draw_torch(self._disturbance_gen, n, dev)
         self.num_steps = torch.zeros(n, dtype=torch.int64, device=dev)
         # zero-copy views of the batch's device buffers
         ptr = eng.device_state_ptrs()
@@ -155,6 +169,24 @@ class DeviceBatchedEnv(envs.BatchedJiminyEnv):
     def _first_command(self) -> None:
         self.engine.set_command(self.sc.target0)
 
+    def _redraw_disturbance(self, done: Optional[torch.Tensor]) -> None:
+        """New disturbance rows for the envs of `done` (None: all), drawn on the device and written by the device setters
+        with the mask in `self._mask`; `disturbance_rows` keeps what every env runs with."""
+        if self.disturbance is None:
+            return
+        new = self.disturbance.draw_torch(self._disturbance_gen, self.n_env, self.torch_device)
+        rows = self.disturbance_rows
+        if done is None:
+            for k in rows:
+                rows[k].copy_(new[k])
+        else:
+            for k in ("t", "dt", "wrench"):
+                sel = done.view(1, -1, *([1] * (rows[k].dim() - 2)))
+                rows[k].copy_(torch.where(sel, new[k], rows[k]))
+            for k in ("values", "grads"):
+                rows[k].copy_(torch.where(done.view(-1, 1), new[k], rows[k]))
+        self.disturbance.apply_device(self.engine, rows, None if done is None else self._mask.data_ptr())
+
     def _restart(self, done: torch.Tensor) -> torch.Tensor:
         """Masked restart of the envs in `done` from bank rows drawn on the device; returns the rows (-1: not restarted)."""
         q_bank, v_bank = self.reset_states
@@ -162,6 +194,7 @@ class DeviceBatchedEnv(envs.BatchedJiminyEnv):
         torch.index_select(q_bank, 0, rows, out=self._q_start)
         torch.index_select(v_bank, 0, rows, out=self._v_start)
         self._mask.copy_(done)
+        self._redraw_disturbance(done)
         self.engine.start_device(self._q_start.data_ptr(), self._v_start.data_ptr(), self._mask.data_ptr())
         self.num_steps.masked_fill_(done, 0)
         return torch.where(done, rows, torch.full_like(rows, -1))
@@ -174,6 +207,7 @@ class DeviceBatchedEnv(envs.BatchedJiminyEnv):
             info: Dict[str, Any] = {}
             if not self._started:
                 self._first_command()
+                self._redraw_disturbance(None)
                 self.engine.start(self.sc.q0, self.sc.v0)
                 self.num_steps.zero_()
                 self._started = True

@@ -16,8 +16,13 @@ timed window (`--duration-max`, default 0.4 s of simulated time).  `--alternate 
 alternating, and reports each loop's spread.  The clock is the host's, around the step loop, ending in a device
 synchronise.
 
+`--disturbance R` turns the walker disturbance on (`std_ratio={"disturbance": R}`: impulses at 2 s intervals of simulated
+time, none within the default `--duration-max`, and the profile evaluated at every dynamics evaluation, re-drawn at every
+restart) and runs each loop with it off and on, alternating in one process, `max(--alternate, 1)` rounds.  External forces
+run the generic kernel, not the quadruped hot path.
+
     python tools/bench_pipeline.py [--robot atlas|anymal] [--loop host|device] [--alternate R] [--n-env 4096]
-                                   [--steps 10] [--warmup 3] [--duration-max 0.4]
+                                   [--steps 10] [--warmup 3] [--duration-max 0.4] [--disturbance R]
 """
 import argparse
 import json
@@ -36,9 +41,10 @@ MAHONY_KP, MAHONY_KI = 0.75, 0.057
 KEYS = [("states", "pd_controller"), ("measurements", "EncoderSensor"), ("features", "mahony_filter")]
 
 
-def make_env(n_env: int, api_=None, robot: str = "atlas", loop: str = "host", duration_max: float = 20.0):
+def make_env(n_env: int, api_=None, robot: str = "atlas", loop: str = "host", duration_max: float = 20.0,
+             disturbance: float = 0.0):
     from jiminy_b200 import envs, scenarios
-    kw = dict(simulation_duration_max=duration_max, api_=api_)
+    kw = dict(simulation_duration_max=duration_max, api_=api_, std_ratio={"disturbance": disturbance} if disturbance > 0 else None)
     if robot == "anymal":
         from jiminy_b200.torch_envs import DeviceBatchedEnv
         return (DeviceBatchedEnv if loop == "device" else envs.BatchedJiminyEnv)(scenarios.make("anymal", n_env, seed=0), **kw)
@@ -71,10 +77,10 @@ def gpu_info() -> dict:
 
 
 def run(n_env: int, steps: int, warmup: int, api_=None, robot: str = "atlas", loop: str = "host",
-        duration_max: float = 0.4) -> dict:
+        duration_max: float = 0.4, disturbance: float = 0.0) -> dict:
     import torch
     from jiminy_b200.envs import flatten_observation
-    env = make_env(n_env, api_, robot, loop, duration_max)
+    env = make_env(n_env, api_, robot, loop, duration_max, disturbance)
     device = loop == "device"
     on_gpu = device and env.torch_device.type == "cuda"
     nm = env.robot.nmotors
@@ -117,7 +123,7 @@ def run(n_env: int, steps: int, warmup: int, api_=None, robot: str = "atlas", lo
             f"contacts, euler_explicit 5 ms" if robot == "atlas" else
             "anymal PD standing (plain PD law), spring-damper contacts, runge_kutta_4 1 ms, per-step position targets")
     out = {"metric": "env_steps_per_sec", "unit": "env-steps/s", "value": n_env * steps / dt, "ms_per_step": 1e3 * dt / steps,
-           "loop": loop, "robot": robot, "n_env": n_env, "steps": steps, "warmup": warmup,
+           "loop": loop, "robot": robot, "disturbance": disturbance, "n_env": n_env, "steps": steps, "warmup": warmup,
            "timing": "host clock around env.step + flatten_observation, ending in a device synchronise",
            "config": {"workload": f"{desc}, {n_env} envs, step_dt {env.step_dt}, simulation_duration_max {duration_max}",
                       "env": type(env).__name__, "lane_plan": env.engine.describe(), "observation_width": int(flat.shape[1])},
@@ -146,6 +152,25 @@ def alternate(rounds: int, **kw) -> dict:
     return out
 
 
+def alternate_disturbance(rounds: int, ratio: float, loops, **kw) -> dict:
+    """Each loop with the disturbance off and on, `rounds` times in this process, alternating; env-steps/s and spread."""
+    runs = {(loop, r): [] for loop in loops for r in (0.0, ratio)}
+    for _ in range(rounds):
+        for loop in loops:
+            for r in (0.0, ratio):
+                runs[(loop, r)].append(run(loop=loop, disturbance=r, **kw))
+    out = {"metric": "env_steps_per_sec", "unit": "env-steps/s", "robot": kw.get("robot", "atlas"), "rounds": rounds}
+    for (loop, r), rs in runs.items():
+        v = sorted(x["value"] for x in rs)
+        out[f"{loop}_disturbance_{'on' if r > 0 else 'off'}"] = {
+            "median": float(np.median(v)), "min": v[0], "max": v[-1], "ms_per_step_median": float(np.median([x["ms_per_step"] for x in rs])),
+            "envs_restarted": [x["envs_restarted"] for x in rs], "envs_flagged": [x["envs_flagged"] for x in rs],
+            "config": rs[-1]["config"]}
+    for loop in loops:
+        out[f"{loop}_on_over_off_median"] = out[f"{loop}_disturbance_on"]["median"] / out[f"{loop}_disturbance_off"]["median"]
+    return out
+
+
 if __name__ == "__main__":
     ap = argparse.ArgumentParser()
     ap.add_argument("--n-env", type=int, default=4096)
@@ -155,8 +180,12 @@ if __name__ == "__main__":
     ap.add_argument("--robot", choices=("atlas", "anymal"), default="atlas")
     ap.add_argument("--alternate", type=int, default=0, metavar="R")
     ap.add_argument("--duration-max", type=float, default=0.4)
+    ap.add_argument("--disturbance", type=float, default=0.0, metavar="R")
     a = ap.parse_args()
     kw = dict(n_env=a.n_env, steps=a.steps, warmup=a.warmup, robot=a.robot, duration_max=a.duration_max)
-    res = alternate(a.alternate, **kw) if a.alternate > 0 else run(loop=a.loop, **kw)
+    if a.disturbance > 0:
+        res = alternate_disturbance(max(a.alternate, 1), a.disturbance, ("host", "device") if a.alternate > 0 else (a.loop,), **kw)
+    else:
+        res = alternate(a.alternate, **kw) if a.alternate > 0 else run(loop=a.loop, **kw)
     res.update(gpu_info())
     print(json.dumps(res))
