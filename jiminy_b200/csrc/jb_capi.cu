@@ -106,6 +106,7 @@ struct JbBatch {
     std::vector<double> h_imp;      // [MAX_IMPULSE][IMPULSE_ROWS][n_pad]
     ExtSlot* d_eslots = nullptr;
     double *d_imp = nullptr, *d_prof_pending = nullptr, *d_prof_latched = nullptr;
+    double* d_latch_snap = nullptr; // latched values at the top of a force-carrying hot-path pass (KParams::latch_snap)
     bool h_imp_stale = false;       // jb_set_impulse_force_device wrote d_imp behind the host mirror
     // process forces: tables [2][ktot][n_pad], host-setter staging [2][n_env][ktot], latched values
     double* d_proc_tab[MAX_PROCESS] = {};
@@ -123,6 +124,7 @@ static int raise_smem_attr(int device, size_t bytes) {
     if (bytes <= g_smem_attr[device]) return JB_OK;
     cudaError_t e = cudaFuncSetAttribute(env_step_kernel_t<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(bytes));
     if (e == cudaSuccess) e = cudaFuncSetAttribute(env_step_kernel_t<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(bytes));
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(env_step_kernel_ext, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(bytes));
     if (e != cudaSuccess) return fail(JB_ERR_CUDA, std::string("cudaFuncSetAttribute: ") + cudaGetErrorString(e));
     g_smem_attr[device] = bytes;
 #endif
@@ -198,10 +200,18 @@ static int ensure_host_stage(JbBatch* b, size_t bytes) {
 static KParams g_kp_on_device[64];
 static bool g_kp_valid[64] = {};
 #endif
+// Do the external forces of this batch ride the hot path (env_step_kernel_ext)?  Quadruped signature, composite-rigid-body
+// evaluation (the ABA sweeps of the signature carry no forces), spring-damper contacts, Euler / RK4.
+static bool forces_on_hot_path(const JbBatch* b) {
+    const KParams& kp = b->kp;
+    return kp.n_eslot > 0 && kp.sig_id == SigQuadruped::ID && kp.rhs_variant == 1 && kp.opt.contact_model == JB_CONTACT_SPRING_DAMPER &&
+           kp.opt.ode_solver != JB_SOLVER_RUNGE_KUTTA_DOPRI && !b->no_fast_kernel;
+}
 static int launch(JbBatch* b, int mode, double step_dt, const uint8_t* d_mask = nullptr, const double* d_command = nullptr,
                   bool validate = false) {
     KParams kp = b->kp;
-    // static plan signatures carry no external-force code
+    // the static plan signatures of the full body carry no external-force code (the force-carrying hot path knows its
+    // signature at compile time)
     if (kp.n_eslot > 0) kp.sig_id = 0;
     LaunchArgs la{};
     la.mode = mode; la.step_dt = step_dt; la.mask = d_mask; la.command = d_command; la.validate = validate ? 1 : 0;
@@ -214,12 +224,14 @@ static int launch(JbBatch* b, int mode, double step_dt, const uint8_t* d_mask = 
     // the hot-path kernel hands envs that leave the hot path over to the full body inside the same launch
     const bool fast = mode == MODE_STEP && kp.n_eslot == 0 && kp.opt.contact_model == JB_CONTACT_SPRING_DAMPER &&
                       kp.opt.ode_solver != JB_SOLVER_RUNGE_KUTTA_DOPRI && !b->no_fast_kernel;
+    const bool fast_ext = mode == MODE_STEP && forces_on_hot_path(b);
     const int epw = 32 / b->plan.L;
     const int nblocks = (b->n_env + epw - 1) / epw;
 #ifdef JB_HOST_EMUL
     emul::current_L = b->plan.L;
     g_kp_host = kp;
     if (fast) JB_LAUNCH(env_step_kernel_t<true>, nblocks, 32, b->smem_bytes, b->stream, la);
+    else if (fast_ext) JB_LAUNCH(env_step_kernel_ext, nblocks, 32, b->smem_bytes, b->stream, la);
     else JB_LAUNCH(env_step_kernel_t<false>, nblocks, 32, b->smem_bytes, b->stream, la);
 #else
     {
@@ -236,6 +248,7 @@ static int launch(JbBatch* b, int mode, double step_dt, const uint8_t* d_mask = 
             ++b->param_uploads;
         }
         if (fast) JB_LAUNCH(env_step_kernel_t<true>, nblocks, 32, b->smem_bytes, b->stream, la);
+        else if (fast_ext) JB_LAUNCH(env_step_kernel_ext, nblocks, 32, b->smem_bytes, b->stream, la);
         else JB_LAUNCH(env_step_kernel_t<false>, nblocks, 32, b->smem_bytes, b->stream, la);
         CU(cudaEventRecord(evt, b->stream));
     }
@@ -610,9 +623,10 @@ int jb_batch_create(const JbModelDesc* m, const JbOptions* opt, int32_t n_env, i
 
 int jb_describe(JbBatch* b, char* buf, int32_t len) {
     if (!b || !buf) return fail(JB_ERR_INVALID_ARGUMENT, "null argument");
-    std::snprintf(buf, len, "%s; hot path: %s%s; constraints: %s", b->plan.describe().c_str(),
+    std::snprintf(buf, len, "%s; hot path: %s%s%s; constraints: %s", b->plan.describe().c_str(),
                   b->kp.sig_id == SigQuadruped::ID ? (b->kp.rhs_variant == 1 ? (b->kp.quad_stage ? "quadruped signature, composite-rigid-body evaluation, one call per RK4 stage" : "quadruped signature, composite-rigid-body evaluation") :"quadruped signature, ABA sweeps") : "ABA sweeps (dynamic plan)",
                   b->kp.fast_bounds ? ", joint bounds solved in the evaluation" : "",
+                  forces_on_hot_path(b) ? ", external forces applied in the evaluation" : "",
                   !b->kp.cons_on ? "flag only" : (b->kp.cq_on ? (b->kp.lb_on ? "structured quadruped solver + lane-block solver" : "structured quadruped solver + generic")
                                                  : (b->kp.bd_on ? "body-space contact solver + lane-block solver" : (b->kp.lb_on ? "lane-block solver" : "generic solver"))));
     for (int j = 0; j < b->kp.n_proc; ++j) {
@@ -1131,9 +1145,11 @@ static int ext_slot_for(JbBatch* b, int joint, const double* p, int* slot_out, b
         if ((rc = dev_alloc(b, &b->d_imp, static_cast<size_t>(MAX_IMPULSE) * IMPULSE_ROWS * N))) return rc;
         if ((rc = dev_alloc(b, &b->d_prof_pending, static_cast<size_t>(MAX_PROFILE) * 6 * N))) return rc;
         if ((rc = dev_alloc(b, &b->d_prof_latched, static_cast<size_t>(MAX_PROFILE) * 6 * N))) return rc;
+        if ((rc = dev_alloc(b, &b->d_latch_snap, static_cast<size_t>(MAX_PROFILE + MAX_PROCESS) * 6 * N))) return rc;
         b->h_imp.assign(static_cast<size_t>(MAX_IMPULSE) * IMPULSE_ROWS * N, 0.0);
         b->kp.eslots = b->d_eslots; b->kp.imp_data = b->d_imp;
         b->kp.prof_pending = b->d_prof_pending; b->kp.prof_latched = b->d_prof_latched;
+        b->kp.latch_snap = b->d_latch_snap;
     }
     // + 1 field behind the slots: the time of the step being taken (stage times of the process forces)
     const size_t smem = static_cast<size_t>(b->base_fields + ESLOT_SIZE * (b->eframes.size() + 1) + 1) * 32 * sizeof(double);

@@ -176,6 +176,9 @@ struct KParams {
     double proc_period[MAX_PROCESS];       // update period: 0 = at every dynamics evaluation
     const double* proc_tab[MAX_PROCESS];
     double* proc_latched;                  // [MAX_PROCESS][6][n_pad]: value held since the last update (finite period)
+    // force-carrying hot path (env_step_kernel_ext): copies of the latched profile / process values taken at the top of the
+    // pass, [MAX_PROFILE + MAX_PROCESS][6][n_pad] (restored on hand-off)
+    double* latch_snap;
 };
 
 // Launch parameters live in constant memory (uniform constant-bank operands in every device
@@ -771,7 +774,7 @@ struct SigDynamic {
 template <bool CONS>
 struct SigQuadrupedT {
     static constexpr int ID = 1;
-    static constexpr bool has_ext = false;   // the host falls back to SigDynamic when forces are registered
+    static constexpr bool has_ext = false;   // forces: SigDynamic in the full body, quadruped_crba<., true> on the hot path
     static constexpr bool has_cons = CONS;   // second instance of the sweeps for `contacts.model = constraint`
     // every lane adds exactly one contribution (its first leg record) to the trunk's pool accumulator: it can be
     // stored instead of zeroed and accumulated
@@ -1543,13 +1546,33 @@ JB_DI void integrate_free_quat(const double* q0, const double* dv, double* q1) {
     q1[3] = q[0] * alpha; q1[4] = q[1] * alpha; q1[5] = q[2] * alpha; q1[6] = q[3] * alpha;
 }
 
+// Impulse / profile / process forces of the slots that record r applies on this lane, subtracted from its bias force f
+// (Engine::computeExternalForces, engine.cc:3455-3495; the same block as in rhs_impl): the world-aligned wrench at the
+// frame origin (xp[0..5]) goes to the joint frame (convertForceGlobalFrameToJoint, utilities/pinocchio.cc:794-809) and is
+// kept in xp[6..11] for the efforts and the extra terms (add_cached_ext_wrench).
+JB_DI void quadruped_ext_wrench(const Ctx& c, const int r, const Xf& oM, Mot& f) {
+    for (int e = 0; e < KP->n_eslot; ++e) {
+        const ExtSlot* es = KP->eslots + (e * 4 + c.sub);
+        if (es->rec != r) continue;
+        double* const xp = jb_smem + (KP->ext_off + ESLOT_SIZE * e) * 32 + c.lane;
+        const V3 Fl = rtmul(oM.R, mk(xp[0], xp[32], xp[64]));
+        const V3 Fa = rtmul(oM.R, mk(xp[96], xp[128], xp[160])) + cross(ld3(es->p), Fl);
+        xp[6 * 32] = Fl.x; xp[7 * 32] = Fl.y; xp[8 * 32] = Fl.z;
+        xp[9 * 32] = Fa.x; xp[10 * 32] = Fa.y; xp[11 * 32] = Fa.z;
+        f.l = f.l - Fl; f.a = f.a - Fa;
+    }
+}
+
 // Evaluation of the quadruped signature in composite-rigid-body form.  STAGE = false: at the stage state already in
 // QS / VS.  STAGE = true: one whole Runge-Kutta stage -- forms the stage state QS = integrate(Q, wq kv), VS = V + wq ka
 // (kv / ka read at the field offsets kv1 / ka1 of the 1-dof records and kvf / kaf of the free-flyer), evaluates there
 // and adds wb (VS, A) to the accumulators (SV, SA) when wb != 0.  The stage state is kept in registers, the contact and
 // the springs take no branch: the base's integrate, the legs' position-only terms and the velocity pass form one basic
 // block that the scheduler interleaves.
-template <bool STAGE>
+// EXT = true: the external-force slots are applied too -- on the base's bias force (record 0: every lane holds the same
+// base record and solves the same base equation, so each applies the wrench once) and on a leg record's before it is
+// stored for the backward recursion (only the lane that owns the joint has ExtSlot::rec == r).
+template <bool STAGE, bool EXT = false>
 JB_DI bool quadruped_crba(const Ctx c, const bool up_to_date, int* status, const double wq, const int kv1, const int ka1,
                           const int kvf, const int kaf, const double wb) {
     using SIG = SigQuadruped;
@@ -1558,6 +1581,13 @@ JB_DI bool quadruped_crba(const Ctx c, const bool up_to_date, int* status, const
     bool out_any = false;
     double qb[7], vb[6], ql[4], vl[4];      // stage state of the free-flyer and of legs records 1..3
     double spk[4] = {0, 0, 0, 0}, spd[4] = {0, 0, 0, 0};
+    int ext_recs = 0;                       // EXT: bit r set when record r applies a force slot on this lane
+    if constexpr (EXT) {
+        for (int e = 0; e < KP->n_eslot; ++e) {
+            const int r = (KP->eslots + (e * 4 + c.sub))->rec;
+            if (r >= 0) ext_recs |= 1 << r;
+        }
+    }
     if constexpr (STAGE) {
         if (KP->springs != nullptr) {
 #pragma unroll
@@ -1610,7 +1640,8 @@ JB_DI bool quadruped_crba(const Ctx c, const bool up_to_date, int* status, const
         const Mot a0 = motion_act_inv(li, g0);          // base acceleration at zero joint acceleration (v x vJ = 0 for the root)
         const double m = K.inertia[0];
         const V3 lc = ld3(K.inertia + 1);
-        const Mot f = inertia_mul(m, lc, K.inertia + 4, a0) + motion_cross_force(v, inertia_mul(m, lc, K.inertia + 4, v));
+        Mot f = inertia_mul(m, lc, K.inertia + 4, a0) + motion_cross_force(v, inertia_mul(m, lc, K.inertia + 4, v));
+        if constexpr (EXT) { if (ext_recs & 1) quadruped_ext_wrench(c, 0, li, f); }   // oMi of the root = liMi
         sm_store_xf(c, RF_LIMI, li);
         sm_store_mot(c, RF_F, f);
         sm_store_mot(c, SIG::imu_off(), v);
@@ -1687,6 +1718,7 @@ JB_DI bool quadruped_crba(const Ctx c, const bool up_to_date, int* status, const
         u += uT;
         RP(R1_U) = sx * u;                               // joint effort along the unsigned axis
         if (!up_to_date) { const double qj = ql[r]; out_any = out_any || K.q_hi < qj || qj < K.q_lo; }
+        if constexpr (EXT) { if ((ext_recs >> r) & 1) quadruped_ext_wrench(c, r, oM, f); }
         sm_store_xf(c, base + R1_LIMI, li);
         sm_store_mot(c, base + R1_FU, f);
         oMc = oM; vc = v; ac = a;
@@ -1873,6 +1905,14 @@ __device__ __noinline__ void stage_quadruped_crba(const Ctx c, const double wq, 
                                                   const int kaf, const double wb, int* status) {
     if (quadruped_crba<true>(c, false, status, wq, kv1, ka1, kvf, kaf, wb)) *status |= ENV_RETRY_FULL;
 }
+// The same two with the external-force slots applied (force-carrying hot path, env_step_kernel_ext)
+__device__ __noinline__ bool rhs_quadruped_crba_ext(const Ctx c, const bool up_to_date, int* status) {
+    return quadruped_crba<false, true>(c, up_to_date, status, 0.0, 0, 0, 0, 0, 0.0);
+}
+__device__ __noinline__ void stage_quadruped_crba_ext(const Ctx c, const double wq, const int kv1, const int ka1, const int kvf,
+                                                      const int kaf, const double wb, int* status) {
+    if (quadruped_crba<true, true>(c, false, status, wq, kv1, ka1, kvf, kaf, wb)) *status |= ENV_RETRY_FULL;
+}
 
 // ------------------------------------------------------------------------------------------
 // Process forces: the wrench of force j at time t, each component a periodic table of knot values and slopes of this env
@@ -1928,6 +1968,14 @@ template <class SIG>
 JB_DI void eval_process_stage(const Ctx& c, double w) {
     if constexpr (sig_has_proc<SIG>::value) eval_process_forces(c, SMF(c, proc_time_field()) + w);
 }
+// The force-carrying hot path of the quadruped signature (env_step_kernel_ext): the plan of SigQuadruped, evaluated by
+// quadruped_crba<., true>, with the process forces of update period 0 at every stage time.  A type of its own, so that
+// the steppers every other batch runs are not touched.
+struct SigQuadrupedExt : SigQuadruped {};
+template <> struct is_fast_quadruped<FastOf<SigQuadrupedExt>> { static constexpr bool value = true; };
+template <> struct sig_has_proc<FastOf<SigQuadrupedExt>> { static constexpr bool value = true; };
+template <class SIG> struct sig_is_fast_ext { static constexpr bool value = false; };
+template <> struct sig_is_fast_ext<FastOf<SigQuadrupedExt>> { static constexpr bool value = true; };
 
 // Engine::computeRobotsDynamics: the sweeps give the unconstrained accelerations; then the constraint path
 // (Engine::computeAcceleration with enabled constraints, engine.cc:3709-3866) corrects them if needed.
@@ -1983,10 +2031,22 @@ JB_DI void rhs_fast(const Ctx c, const bool up_to_date, int* status) {
                          : rhs_dynamic<false>(c, up_to_date, status);
     if (out) *status |= ENV_RETRY_FULL;
 }
+// force-carrying hot path: the quadruped signature's composite-rigid-body evaluation with the force slots
+JB_DI void rhs_fast_ext(const Ctx c, const bool up_to_date, int* status) {
+    if (rhs_quadruped_crba_ext(c, up_to_date, status)) *status |= ENV_RETRY_FULL;
+}
 template <class SIG>
 JB_DI void rhs_sig(const Ctx c, const bool up_to_date, int* status) {
-    if constexpr (sig_is_fast<SIG>::value) rhs_fast(c, up_to_date, status);
+    if constexpr (sig_is_fast_ext<SIG>::value) rhs_fast_ext(c, up_to_date, status);
+    else if constexpr (sig_is_fast<SIG>::value) rhs_fast(c, up_to_date, status);
     else rhs(c, up_to_date, status);
+}
+// one-call RK4 stage of the quadruped hot path, with or without the force slots
+template <class SIG>
+JB_DI void stage_quadruped_sig(const Ctx c, const double wq, const int kv1, const int ka1, const int kvf, const int kaf,
+                               const double wb, int* status) {
+    if constexpr (sig_is_fast_ext<SIG>::value) stage_quadruped_crba_ext(c, wq, kv1, ka1, kvf, kaf, wb, status);
+    else stage_quadruped_crba(c, wq, kv1, ka1, kvf, kaf, wb, status);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -2202,8 +2262,9 @@ __device__ __noinline__ void step_rk4_t(const Ctx c, double dt, int* status) {
         const double w = dt * (i == 3 ? 1.0 : 0.5);
         if constexpr (quad_fast) {
             if (one_call) {
-                stage_quadruped_crba(c, w, i == 1 ? R1_V : R1_VS, R1_A, i == 1 ? RF_V : RF_VS, RF_A,
-                                     dt * (i == 3 ? 1.0 / 6.0 : 1.0 / 3.0), status);
+                eval_process_stage<SIG>(c, w);
+                stage_quadruped_sig<SIG>(c, w, i == 1 ? R1_V : R1_VS, R1_A, i == 1 ? RF_V : RF_VS, RF_A,
+                                         dt * (i == 3 ? 1.0 / 6.0 : 1.0 / 3.0), status);
                 continue;
             }
         }
@@ -2229,7 +2290,7 @@ __device__ __noinline__ void step_rk4_t(const Ctx c, double dt, int* status) {
     }
     // candidate solution = x0 (+) sum ; it is always accepted, then dx = f(t + dt, x)
     if constexpr (quad_fast) {
-        if (one_call) stage_quadruped_crba(c, 1.0, R1_SV, R1_SA, RF_SV, RF_SA, 0.0, status);
+        if (one_call) { eval_process_stage<SIG>(c, dt); stage_quadruped_sig<SIG>(c, 1.0, R1_SV, R1_SA, RF_SV, RF_SA, 0.0, status); }
         else make_stage<SIG>(c, 1.0, R1_SV, R1_SA, RF_SV, RF_SA);
     } else {
         make_stage<SIG>(c, 1.0, R1_SV, R1_SA, RF_SV, RF_SA);
@@ -2250,22 +2311,30 @@ __device__ __noinline__ void step_rk4_t(const Ctx c, double dt, int* status) {
             RP(R1_V) = RP(R1_VS);
         }
     });
-    eval_process_stage<SIG>(c, dt);
-    if (!one_call) rhs_sig<SIG>(c, false, status);
+    if (!one_call) {
+        eval_process_stage<SIG>(c, dt);
+        rhs_sig<SIG>(c, false, status);
+    }
 }
 
-// run-time dispatch on the plan signature
+// run-time dispatch on the plan signature (QUAD: the quadruped signature whatever sig_id says -- the force-carrying
+// hot path, whose batches keep sig_id = 0 for the full body)
+template <bool QUAD = false>
 JB_DI void stage_from_accepted(const Ctx& c) {
-    if (KP->sig_id == SigQuadruped::ID) stage_from_accepted_t<SigQuadruped>(c);
+    if (QUAD || KP->sig_id == SigQuadruped::ID) stage_from_accepted_t<SigQuadruped>(c);
     else stage_from_accepted_t<SigDynamic<false>>(c);
 }
+template <bool QUAD = false>
 JB_DI bool accel_has_nan(const Ctx& c) {
-    if (KP->sig_id == SigQuadruped::ID) return accel_has_nan_t<SigQuadruped>(c);
+    if (QUAD || KP->sig_id == SigQuadruped::ID) return accel_has_nan_t<SigQuadruped>(c);
     return accel_has_nan_t<SigDynamic<false>>(c);
 }
-template <bool FAST>
+// EXT (with FAST): the force-carrying hot path, quadruped signature only
+template <bool FAST, bool EXT = false>
 JB_DI void step_euler(const Ctx c, double dt, int* status) {
-    if constexpr (FAST) {
+    if constexpr (EXT) {
+        step_euler_t<FastOf<SigQuadrupedExt>>(c, dt, status);
+    } else if constexpr (FAST) {
         if (KP->sig_id == SigQuadruped::ID) step_euler_t<FastOf<SigQuadruped>>(c, dt, status);
         else step_euler_t<FastOf<SigDynamic<false>>>(c, dt, status);
     } else {
@@ -2274,9 +2343,11 @@ JB_DI void step_euler(const Ctx c, double dt, int* status) {
         else step_euler_t<SigDynamic<false>>(c, dt, status);
     }
 }
-template <bool FAST>
+template <bool FAST, bool EXT = false>
 JB_DI void step_rk4(const Ctx c, double dt, int* status) {
-    if constexpr (FAST) {
+    if constexpr (EXT) {
+        step_rk4_t<FastOf<SigQuadrupedExt>>(c, dt, status);
+    } else if constexpr (FAST) {
         if (KP->sig_id == SigQuadruped::ID) step_rk4_t<FastOf<SigQuadruped>>(c, dt, status);
         else step_rk4_t<FastOf<SigDynamic<false>>>(c, dt, status);
     } else {

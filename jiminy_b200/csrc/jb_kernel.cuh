@@ -196,6 +196,23 @@ __device__ __noinline__ void snapshot_blocks(const Ctx c, const int L, const boo
     jb_syncwarp(c);
 }
 
+// The same for the latched values of the profile / process forces with a finite update period (force-carrying hot path):
+// an update hit inside a pass that is handed over overwrites the value the replay starts from.
+__device__ __noinline__ void snapshot_latched(const Ctx c, const int L, const bool restore) {
+    if (restore) jb_syncwarp(c);   // sub-lane 0 wrote the live values
+    const size_t N = KP->n_pad, col = c.env;
+    for (int k = c.sub; k < 6 * (KP->n_prof + KP->n_proc); k += L) {
+        const int j = k / 6, i = k % 6;
+        const bool prof = j < KP->n_prof;
+        if (!((prof ? KP->prof_period[j] : KP->proc_period[j - KP->n_prof]) > D_EPS)) continue;
+        double* live = (prof ? KP->prof_latched + static_cast<size_t>(j) * 6 * N
+                             : KP->proc_latched + static_cast<size_t>(j - KP->n_prof) * 6 * N) + i * N + col;
+        double* snap = KP->latch_snap + (static_cast<size_t>(j) * 6 + i) * N + col;
+        if (restore) *live = *snap; else *snap = *live;
+    }
+    jb_syncwarp(c);
+}
+
 __device__ __noinline__ void store_outputs(const Ctx c) {
     if (!c.valid) return;
     const int L = KP->L;
@@ -347,8 +364,12 @@ __device__ __noinline__ void store_dynamics(const Ctx c) {
 #define JB_EMUL_LEAVES_EARLY(pass)
 #endif
 
-template <bool FAST>
+// EXT = true (with FAST): the force-carrying hot path of the quadruped signature (env_step_kernel_ext).  Everything the
+// full body does for impulse / profile / process forces runs here too: slots zeroed at load, refreshed at every
+// scheduler iteration (impulse breakpoints, FSAL repair on a change), process forces before every evaluation.
+template <bool FAST, bool EXT = false>
 __device__ __forceinline__ void env_step_body(const LaunchArgs& la, const bool only_flagged) {
+    static_assert(FAST || !EXT, "external forces on the full body need no instance of their own");
     Ctx c;
     c.lane = threadIdx.x & 31;
     const int L = KP->L;
@@ -398,6 +419,9 @@ __device__ __forceinline__ void env_step_body(const LaunchArgs& la, const bool o
     if constexpr (FAST) {
         if (c.valid && (KP->pdf != nullptr || KP->mahony != nullptr || KP->sp_on)) snapshot_blocks(c, L, false);
     }
+    if constexpr (EXT) {
+        if (c.valid && KP->n_prof + KP->n_proc > 0) snapshot_latched(c, L, false);
+    }
     // ---------------- load state into the lane records
     for (int r = 0; r < KP->nrec; ++r) {
         const RecInt* ri = KP->rint + (r * L + c.sub);
@@ -430,8 +454,10 @@ __device__ __forceinline__ void env_step_body(const LaunchArgs& la, const bool o
             SMF(c, KP->rec_off[1] + R1_BFAIL) = CST(CS_SOLVE_FAILED);
         }
     }
-    if constexpr (!FAST) {
+    if constexpr (!FAST || EXT) {
         for (int k = 0; k < ESLOT_SIZE * KP->n_eslot; ++k) SMF(c, KP->ext_off + k) = 0.0;
+    }
+    if constexpr (!FAST) {
         if (KP->cons_on) {
             if (mode == MODE_STEP) cons_load_count(c);
             else SMF(c, KP->cons_off) = 0.0;
@@ -523,16 +549,18 @@ __device__ __forceinline__ void env_step_body(const LaunchArgs& la, const bool o
             double solveFailedBackup = 0.0;
             if constexpr (!FAST) {
                 if (KP->cons_on) solveFailedBackup = CST(CS_SOLVE_FAILED);
+            }
+            if constexpr (!FAST || EXT) {
                 if (KP->n_proc > 0) SMF(c, proc_time_field()) = t;   // stage times of the process forces
             }
-            if (opt.ode_solver == JB_SOLVER_EULER_EXPLICIT) { step_euler<FAST>(c, dtLargest, &status); dtLargest = D_INF; }
-            else if (FAST || opt.ode_solver == JB_SOLVER_RUNGE_KUTTA_4) { step_rk4<FAST>(c, dtLargest, &status); dtLargest = D_INF; }
+            if (opt.ode_solver == JB_SOLVER_EULER_EXPLICIT) { step_euler<FAST, EXT>(c, dtLargest, &status); dtLargest = D_INF; }
+            else if (FAST || opt.ode_solver == JB_SOLVER_RUNGE_KUTTA_4) { step_rk4<FAST, EXT>(c, dtLargest, &status); dtLargest = D_INF; }
             else { if constexpr (!FAST) rc = step_dopri(c, &dtLargest, &status); }
             need_refresh = false;
             if constexpr (FAST) {
                 // one vote for the two rare events of a step: NaN in the new acceleration, or a joint that left its
                 // position bounds (this env is then re-done by the full kernel)
-                const bool bad = accel_has_nan(c), retry = (status & ENV_RETRY_FULL) != 0;
+                const bool bad = accel_has_nan<EXT>(c), retry = (status & ENV_RETRY_FULL) != 0;
                 if (jb_any(c, bad || retry)) {
                     if (jb_any(c, retry)) { status |= ENV_RETRY_FULL; failed = true; }
                     if (jb_any(c, bad)) rc = 2;
@@ -571,7 +599,7 @@ __device__ __forceinline__ void env_step_body(const LaunchArgs& la, const bool o
             double tNext = t;
             // impulse forces: active set + next breakpoint; profile forces: held values (engine.cc:1843-1917)
             double tImpulseForceNext = D_INF;
-            if constexpr (!FAST) { if (KP->n_eslot > 0) tImpulseForceNext = refresh_external_forces(c, t, false, finitePeriod, hasDynamicsChanged); }
+            if constexpr (!FAST || EXT) { if (KP->n_eslot > 0) tImpulseForceNext = refresh_external_forces(c, t, false, finitePeriod, hasDynamicsChanged); }
             if (finitePeriod && opt.controller_update_period > D_EPS) {
                 if (period_hit(t, opt.controller_update_period)) {
                     // computeCommand (engine.cc:1920-1940): zero-order hold of the action, or the PD block
@@ -580,9 +608,10 @@ __device__ __forceinline__ void env_step_body(const LaunchArgs& la, const bool o
                 }
             }
             if (!finitePeriod && hasDynamicsChanged) {
-                stage_from_accepted(c);
-                if constexpr (!FAST) { if (KP->n_proc > 0) eval_process_forces(c, t); }
-                if constexpr (FAST) rhs_fast(c, !need_refresh, &status); else rhs(c, !need_refresh, &status);
+                stage_from_accepted<EXT>(c);
+                if constexpr (!FAST || EXT) { if (KP->n_proc > 0) eval_process_forces(c, t); }
+                if constexpr (EXT) rhs_fast_ext(c, !need_refresh, &status);
+                else if constexpr (FAST) rhs_fast(c, !need_refresh, &status); else rhs(c, !need_refresh, &status);
                 need_refresh = false;
                 hasDynamicsChanged = false;
             }
@@ -596,9 +625,10 @@ __device__ __forceinline__ void env_step_body(const LaunchArgs& la, const bool o
                 while (tNext - t > STEPPER_MIN_TIMESTEP && !failed) {
                     if (hasDynamicsChanged) {
                         // FSAL repair: same state, cached contact forces, new command (engine.cc:2032-2037)
-                        stage_from_accepted(c);
-                        if constexpr (!FAST) { if (KP->n_proc > 0) eval_process_forces(c, t); }
-                        if constexpr (FAST) rhs_fast(c, !need_refresh, &status); else rhs(c, !need_refresh, &status);
+                        stage_from_accepted<EXT>(c);
+                        if constexpr (!FAST || EXT) { if (KP->n_proc > 0) eval_process_forces(c, t); }
+                        if constexpr (EXT) rhs_fast_ext(c, !need_refresh, &status);
+                        else if constexpr (FAST) rhs_fast(c, !need_refresh, &status); else rhs(c, !need_refresh, &status);
                         need_refresh = false;
                         hasDynamicsChanged = false;
                     }
@@ -648,6 +678,7 @@ __device__ __forceinline__ void env_step_body(const LaunchArgs& la, const bool o
     if constexpr (FAST) {
         if (jb_any(c, (status & ENV_RETRY_FULL) != 0)) {   // nothing of this pass is kept: the full body redoes the env
             if (c.valid && (KP->pdf != nullptr || KP->mahony != nullptr || KP->sp_on)) snapshot_blocks(c, L, true);
+            if constexpr (EXT) { if (c.valid && KP->n_prof + KP->n_proc > 0) snapshot_latched(c, L, true); }
             if (c.sub == 0) *needs_full = 1;
             return;
         }
@@ -740,12 +771,12 @@ __device__ __noinline__ void env_step_full(const LaunchArgs la, const bool only_
 
 // One launch = one Engine::step (or start / single evaluation) of every env.  FAST: the hot-path body first; the envs it
 // handed over (a joint left its bounds now, or constraints still enabled from an earlier step) go through the full
-// body in the same launch, so a step is always exactly one kernel.
-template <bool FAST>
-__global__ void __launch_bounds__(32) env_step_kernel_t(const LaunchArgs la) {
+// body in the same launch, so a step is always exactly one kernel.  EXT: the hot-path body is the force-carrying one.
+template <bool FAST, bool EXT>
+__device__ __forceinline__ void env_step_launch(const LaunchArgs& la) {
     JB_PROF_T(t_kernel);
     if constexpr (FAST) {
-        env_step_body<true>(la, false);
+        env_step_body<true, EXT>(la, false);
         __syncwarp();   // needs_full is written by sub-lane 0 of each env
         const int flag = KP->needs_full[blockIdx.x * (32 / KP->L) + (threadIdx.x & 31) / KP->L];
         if (__any_sync(0xffffffffu, flag != 0)) env_step_full(la, true);
@@ -769,6 +800,11 @@ __global__ void __launch_bounds__(32) env_step_kernel_t(const LaunchArgs la) {
     }
 #endif
 }
+template <bool FAST>
+__global__ void __launch_bounds__(32) env_step_kernel_t(const LaunchArgs la) { env_step_launch<FAST, false>(la); }
+// Batches of the quadruped signature with external forces (composite-rigid-body evaluation, spring-damper contacts,
+// Euler / RK4): the forces ride the hot path, the envs it hands over run the full body's force-aware generic sweeps.
+__global__ void __launch_bounds__(32) env_step_kernel_ext(const LaunchArgs la) { env_step_launch<true, true>(la); }
 
 // ---- observation exchange over peer memory: the consumer's wait (one thread)
 #ifndef JB_HOST_EMUL

@@ -18,8 +18,8 @@ synchronise.
 
 `--disturbance R` turns the walker disturbance on (`std_ratio={"disturbance": R}`: impulses at 2 s intervals of simulated
 time, none within the default `--duration-max`, and the profile evaluated at every dynamics evaluation, re-drawn at every
-restart) and runs each loop with it off and on, alternating in one process, `max(--alternate, 1)` rounds.  External forces
-run the generic kernel, not the quadruped hot path.
+restart) and runs each loop with it off and on, alternating in one process, `max(--alternate, 1)` rounds.  On ANYmal the
+forces ride the quadruped hot path (`env_step_kernel_ext`); Atlas runs the generic kernel either way.
 
     python tools/bench_pipeline.py [--robot atlas|anymal] [--loop host|device] [--alternate R] [--n-env 4096]
                                    [--steps 10] [--warmup 3] [--duration-max 0.4] [--disturbance R]

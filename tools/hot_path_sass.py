@@ -2,7 +2,9 @@
 """Static SASS summary of the quadruped hot path in the step kernel (env_step_kernel_t<true>): for the RK4 step of the
 quadruped signature, the composite-rigid-body evaluation and the one-call RK4 stage, print the instruction count, the
 FP64 instruction count, basic blocks, local-memory traffic (STL / LDL), calls into the library's division / square-root
-/ trigonometric slow paths, and the spills ptxas reports.
+/ trigonometric slow paths, and the spills ptxas reports.  The rows below them are the same functions of the
+force-carrying hot path (env_step_kernel_ext: the RK4 and Euler steps, the evaluation and the stage with the external-force
+slots applied).
 
 Usage: python tools/hot_path_sass.py [--lib LIB.so [--ptxas-log LOG]]
 Without --lib the library is compiled from the tree into a temporary directory (with -Xptxas -v, for the spills).
@@ -17,9 +19,14 @@ import tempfile
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 KERNEL = "_ZN2jb17env_step_kernel_tILb1EEEvNS_10LaunchArgsE"
-FUNCS = [("step_rk4_t<FastOf<SigQuadruped>>", "_ZN2jb10step_rk4_tINS_6FastOfINS_13SigQuadrupedTILb0EEEEEEEvNS_3CtxEdPi"),
-         ("rhs_quadruped_crba", "_ZN2jb18rhs_quadruped_crbaENS_3CtxEbPi"),
-         ("stage_quadruped_crba", "_ZN2jb20stage_quadruped_crbaENS_3CtxEdiiiidPi")]
+KERNEL_EXT = "_ZN2jb19env_step_kernel_extENS_10LaunchArgsE"
+FUNCS = [("step_rk4_t<FastOf<SigQuadruped>>", KERNEL, "_ZN2jb10step_rk4_tINS_6FastOfINS_13SigQuadrupedTILb0EEEEEEEvNS_3CtxEdPi"),
+         ("rhs_quadruped_crba", KERNEL, "_ZN2jb18rhs_quadruped_crbaENS_3CtxEbPi"),
+         ("stage_quadruped_crba", KERNEL, "_ZN2jb20stage_quadruped_crbaENS_3CtxEdiiiidPi"),
+         ("step_rk4_t<FastOf<SigQuadrupedExt>>", KERNEL_EXT, "_ZN2jb10step_rk4_tINS_6FastOfINS_15SigQuadrupedExtEEEEEvNS_3CtxEdPi"),
+         ("step_euler_t<FastOf<SigQuadrupedExt>>", KERNEL_EXT, "_ZN2jb12step_euler_tINS_6FastOfINS_15SigQuadrupedExtEEEEEvNS_3CtxEdPi"),
+         ("rhs_quadruped_crba_ext", KERNEL_EXT, "_ZN2jb22rhs_quadruped_crba_extENS_3CtxEbPi"),
+         ("stage_quadruped_crba_ext", KERNEL_EXT, "_ZN2jb24stage_quadruped_crba_extENS_3CtxEdiiiidPi")]
 FP64 = {"DFMA", "DMUL", "DADD", "DSETP", "DMNMX"}
 
 
@@ -53,8 +60,8 @@ def disassemble(lib, tmp):
     return subprocess.run(["nvdisasm", "-c", cubin], capture_output=True, text=True, check=True).stdout.splitlines()
 
 
-def body(lines, mangled):
-    head = f"${KERNEL}${mangled}:"
+def body(lines, kernel, mangled):
+    head = f"${kernel}${mangled}:"
     try:
         start = lines.index(head)
     except ValueError:
@@ -90,15 +97,15 @@ def main():
     sp = spills(log) if log is not None else {}
     print(f"library: {lib}")
     cols = ["instructions", "fp64", "basic_blocks", "STL", "LDL", "slow_path_calls", "trig_calls", "spill_bytes"]
-    print(f"{'function':<34}" + "".join(f"{c:>16}" for c in cols))
-    for name, mangled in FUNCS:
-        fn = body(lines, mangled)
+    print(f"{'function':<38}" + "".join(f"{c:>16}" for c in cols))
+    for name, kernel, mangled in FUNCS:
+        fn = body(lines, kernel, mangled)
         if fn is None:
-            print(f"{name:<34}  (not in this library)")
+            print(f"{name:<38}  (not in this library)")
             continue
         s = summary(fn)
         s["spill_bytes"] = sp.get(mangled, "n/a")
-        print(f"{name:<34}" + "".join(f"{s[c]:>16}" for c in cols) + f"   {s['calls_by_target']}")
+        print(f"{name:<38}" + "".join(f"{s[c]:>16}" for c in cols) + f"   {s['calls_by_target']}")
 
 
 if __name__ == "__main__":
