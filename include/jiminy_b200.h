@@ -376,6 +376,31 @@ int jb_set_sensor_options(JbBatch* batch, int32_t type, int32_t index, const dou
  * (abstract_sensor.hxx:213-226, random.cc:10-37).  Default: 0 for every env. */
 int jb_set_seeds(JbBatch* batch, const uint32_t* seeds /* [n_env] */);
 int jb_get_sensor_data(JbBatch* batch, double* out /* [n_env][width] true values */);
+/* Per-env sensor options: what the walker env's setOptions of every sensor at every reset needs (gym_jiminy
+ * locomotion.py:264-286), with envs restarting while others run.  jb_enable_per_env_sensor_options puts every sensor in
+ * the measurement pipeline with per-env option tables (initially all zero; noise and bias are applied for every sensor,
+ * delayInterpolationOrder 1) and sizes the delay ring once for `delay_bound`, the largest delay + jitter any row may hold.
+ * Only between episodes, like jb_set_sensor_options, which it replaces: afterwards that one returns JB_ERR_BAD_CONTROL_FLOW.
+ * Needs a discrete sensorsUpdatePeriod.
+ * jb_set_sensor_options_env writes the rows of the envs selected by mask (NULL = all): noise_std and bias [n_env][width]
+ * in the columns of the sensor matrix (jb_sensor_layout), one value per field of every sensor; delay and jitter
+ * [n_env][nsensors] in the pipeline's sensor order (Imu, Force, Encoder, Effort, Contact; attach order within a type).
+ * The rows are pending: an env runs with them from its next start (jb_start with the env in its mask, or
+ * jb_start_device), which also computes that env's per-type delayMax; a running env is not affected, as a locked robot
+ * refuses setOptions in the reference.  A row with a NaN, a negative delay or jitter, or delay + jitter > delay_bound is
+ * refused: the host form writes nothing and returns JB_ERR_INVALID_ARGUMENT naming the env; the _device form (device
+ * buffers, one kernel on the batch stream, no host synchronisation) skips that row and marks the env, whose starts then
+ * leave it JB_ENV_NOT_STARTED | JB_ENV_BAD_START until a valid row for it is written. */
+int jb_enable_per_env_sensor_options(JbBatch* batch, double delay_bound);
+int jb_set_sensor_options_env(JbBatch* batch, const uint8_t* mask, const double* noise_std, const double* bias,
+                              const double* delay, const double* jitter);
+int jb_set_sensor_options_env_device(JbBatch* batch, const uint8_t* mask_dev, const double* noise_std_dev,
+                                     const double* bias_dev, const double* delay_dev, const double* jitter_dev);
+/* jb_set_seeds for the envs selected by mask_dev (NULL = all) from a device buffer seeds_dev [n_env], one kernel on the
+ * batch stream: the generator start states of those envs, bit-identical to the ones jb_set_seeds + jb_start derive on the
+ * host.  The host does not overwrite them from its own copy of the seeds until the next jb_set_seeds.  Needs the
+ * measurement pipeline (a sensor option, or per-env options). */
+int jb_set_seeds_device(JbBatch* batch, const uint8_t* mask_dev, const uint32_t* seeds_dev);
 
 /* Replaces: the quantities Engine::computeExtraTerms leaves in pinocchio::Data after each
  * successful step (engine.cc:800-905): per env kinetic+potential energy `energy` [n_env][2],

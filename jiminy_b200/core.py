@@ -66,7 +66,8 @@ class Api:
                "jb_set_sensor_options", "jb_set_seeds", "jb_get_sensor_data",
                "jb_start_device", "jb_set_pd_adapter", "jb_pd_adapter_device", "jb_device_block_views",
                "jb_set_impulse_force_device", "jb_register_process_force", "jb_set_process_force",
-               "jb_set_process_force_device")
+               "jb_set_process_force_device", "jb_enable_per_env_sensor_options", "jb_set_sensor_options_env",
+               "jb_set_sensor_options_env_device", "jb_set_seeds_device")
 
     def __init__(self, cdll: C.CDLL):
         self.dll = L = cdll
@@ -138,6 +139,10 @@ class Api:
                                                 c_double_p, c_int32_p]
         L.jb_set_process_force.argtypes = [vp, C.c_int32, c_uint8_p, c_double_p, c_double_p]
         L.jb_set_process_force_device.argtypes = [vp, C.c_int32, vp, vp, vp]
+        L.jb_enable_per_env_sensor_options.argtypes = [vp, C.c_double]
+        L.jb_set_sensor_options_env.argtypes = [vp, c_uint8_p] + [c_double_p] * 4
+        L.jb_set_sensor_options_env_device.argtypes = [vp] + [vp] * 5
+        L.jb_set_seeds_device.argtypes = [vp, vp, vp]
 
     def check(self, rc: int) -> None:
         if rc != JB_OK:
@@ -504,6 +509,43 @@ class BatchedEngine:
         s = np.ascontiguousarray(seeds, dtype=np.uint32)
         assert s.shape == (self.n_env,)
         self._api.check(self._api.dll.jb_set_seeds(self._h, s.ctypes.data_as(C.POINTER(C.c_uint32))))
+
+    def set_seeds_device(self, seeds_ptr: int, mask_ptr: Optional[int] = None) -> None:
+        """`set_seeds` for the envs of `mask` (None = all) from a device buffer (seeds [n_env] uint32, or int32 with the
+        same bits), enqueued on the batch stream with no host synchronisation: the generator start states of those envs
+        are derived on the device, bit-identical to the host derivation."""
+        self._api.check(self._api.dll.jb_set_seeds_device(self._h, C.c_void_p(mask_ptr or None), C.c_void_p(seeds_ptr)))
+
+    def enable_per_env_sensor_options(self, delay_bound: float) -> None:
+        """Per-env options for every sensor (`set_sensor_options_env`), all zero until set, in place of the batch-wide
+        `set_sensor_options`.  `delay_bound`: the largest delay + jitter any row may hold (sizes the delay buffer)."""
+        self._api.check(self._api.dll.jb_enable_per_env_sensor_options(self._h, float(delay_bound)))
+
+    @property
+    def n_sensors(self) -> int:
+        """Sensors of the measurement pipeline: the rows of `delay` / `jitter` in `set_sensor_options_env`."""
+        return sum(self.robot.sensor_layout()[t][2] for t in self.SENSOR_TYPES)
+
+    def set_sensor_options_env(self, noise_std, bias, delay, jitter, mask: Optional[np.ndarray] = None) -> None:
+        """Per-env options of the envs of `mask` (None = all): noise_std, bias [n_env, width] in the columns of the sensor
+        matrix, delay, jitter [n_env, n_sensors] in the order Imu, Force, Encoder, Effort, Contact.  They apply from each
+        env's next start.  A row with a NaN, a negative delay or jitter, or delay + jitter beyond the bound raises
+        ValueError and nothing is written."""
+        ns = self.n_sensors
+        noise_std, bias = self._per_env(noise_std, (self.width,)), self._per_env(bias, (self.width,))
+        delay, jitter = self._per_env(delay, (ns,)), self._per_env(jitter, (ns,))
+        m = None if mask is None else np.ascontiguousarray(mask, dtype=np.uint8)
+        self._api.check(self._api.dll.jb_set_sensor_options_env(
+            self._h, None if m is None else m.ctypes.data_as(c_uint8_p), dptr(noise_std), dptr(bias), dptr(delay), dptr(jitter)))
+
+    def set_sensor_options_env_device(self, noise_std_ptr: int, bias_ptr: int, delay_ptr: int, jitter_ptr: int,
+                                      mask_ptr: Optional[int] = None) -> None:
+        """`set_sensor_options_env` from device buffers of the same layouts (fp64; mask [n_env] uint8 or None), enqueued on
+        the batch stream with no host synchronisation.  A rejected row is not written and its env stays
+        JB_ENV_NOT_STARTED | JB_ENV_BAD_START through its starts until a valid row for it arrives."""
+        self._api.check(self._api.dll.jb_set_sensor_options_env_device(
+            self._h, C.c_void_p(mask_ptr or None), C.c_void_p(noise_std_ptr), C.c_void_p(bias_ptr), C.c_void_p(delay_ptr),
+            C.c_void_p(jitter_ptr)))
 
     def get_sensor_data(self) -> np.ndarray:
         out = np.zeros((self.n_env, max(self.width, 1)))

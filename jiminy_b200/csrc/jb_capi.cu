@@ -74,6 +74,12 @@ struct JbBatch {
     unsigned long long *d_sp_rng = nullptr, *d_sp_rng_init = nullptr, *d_sp_snap_rng = nullptr;
     int32_t *d_sp_count = nullptr, *d_sp_snap_count = nullptr;
     double *d_sp_times = nullptr, *d_sp_ring = nullptr, *d_sens_true = nullptr;
+    // per-env sensor options (jb_enable_per_env_sensor_options): pending / latched rows, host-setter staging, reject flags
+    bool sp_env = false;
+    double sp_env_bound = 0.0;     // largest delay + jitter a row may hold (sizes the delay ring)
+    double *d_sp_env_pending = nullptr, *d_sp_env_opt = nullptr, *d_sp_env_stage = nullptr;
+    int32_t* d_sp_env_bad = nullptr;
+    bool sp_seeds_dev = false;     // jb_set_seeds_device wrote generator start states the host's seeds no longer describe
     double *d_cmd_dyn = nullptr, *d_cstate_save = nullptr;   // jb_compute_dynamics: command of the evaluation, saved constraint state
     int nimu = 0;
     uint8_t* d_mask = nullptr;
@@ -923,6 +929,7 @@ int jb_set_sensor_options(JbBatch* b, int32_t type, int32_t index, const double*
     if (delay_interpolation_order != 0 && delay_interpolation_order != 1) return fail(JB_ERR_NOT_IMPLEMENTED, "`delayInterpolationOrder` must be either 0 or 1.");
     if (!(b->kp.opt.sensors_update_period > 2.3e-16))
         return fail(JB_ERR_NOT_IMPLEMENTED, "the device measurement pipeline needs a discrete sensorsUpdatePeriod (the delay buffer is sized from it)");
+    if (b->sp_env) return fail(JB_ERR_BAD_CONTROL_FLOW, "per-env sensor options are enabled: set them with jb_set_sensor_options_env");
     if (b->sdesc.empty()) {
         for (int ty = 0; ty < 5; ++ty)
             for (int k = 0; k < counts[ty]; ++k) {
@@ -946,18 +953,17 @@ int jb_set_seeds(JbBatch* b, const uint32_t* seeds) {
     if (!b || !seeds) return fail(JB_ERR_INVALID_ARGUMENT, "null argument");
     b->seeds.assign(seeds, seeds + b->n_env);
     b->sp_rows_dirty = true;
+    b->sp_seeds_dev = false;
     return JB_OK;
 }
 
-// Tables, buffers and start states of the pipeline, (re)built at jb_start when options changed.  `rows_if_dirty`
-// (jb_start_device, which has no host mask): the generator start states of ALL envs, and only when the seeds or the
-// sensor set changed since they were last uploaded -- the kernel reads an env's row only when that env (re)starts.
-static int prepare_sensor_pipeline(JbBatch* b, const uint8_t* mask, bool rows_if_dirty = false) {
-    if (b->sdesc.empty()) return JB_OK;
+// Tables and buffers of the pipeline, (re)built when the options changed: descriptors, generator states, the delay ring
+// sized for the largest delay + jitter (per-env options: the declared bound) and the ziggurat tables.
+static int build_sensor_tables(JbBatch* b) {
     KParams& kp = b->kp;
     const int ns = static_cast<int>(b->sdesc.size());
-    if (b->sp_dirty || !kp.sp_on) {
-        double dmax_all = 0.0;
+    {
+        double dmax_all = b->sp_env ? b->sp_env_bound : 0.0;
         for (int ty = 0; ty < 5; ++ty) kp.sp_delay_max[ty] = 0.0;
         for (const SensorDesc& d : b->sdesc) {
             kp.sp_delay_max[d.type] = std::max(kp.sp_delay_max[d.type], d.delay + d.jitter);
@@ -1011,6 +1017,22 @@ static int prepare_sensor_pipeline(JbBatch* b, const uint8_t* mask, bool rows_if
         kp.sp_count = b->d_sp_count; kp.sp_snap_count = b->d_sp_snap_count; kp.sp_times = b->d_sp_times; kp.sp_ring = b->d_sp_ring;
         b->sp_dirty = false;
     }
+    return JB_OK;
+}
+
+// Tables rebuilt when options changed, then the generator start states at jb_start.  `rows_if_dirty` (jb_start_device,
+// which has no host mask): the start states of ALL envs, and only when the seeds or the sensor set changed since they
+// were last uploaded -- the kernel reads an env's row only when that env (re)starts.  After jb_set_seeds_device the
+// device rows are the only up-to-date ones: nothing is uploaded until the next jb_set_seeds.
+static int prepare_sensor_pipeline(JbBatch* b, const uint8_t* mask, bool rows_if_dirty = false) {
+    if (b->sdesc.empty()) return JB_OK;
+    KParams& kp = b->kp;
+    const int ns = static_cast<int>(b->sdesc.size());
+    if (b->sp_dirty || !kp.sp_on) {
+        int rc = build_sensor_tables(b);
+        if (rc) return rc;
+    }
+    if (b->sp_seeds_dev) return JB_OK;
     // Start states of the generators: Engine::reset seeds the engine's PCG32 from stepper.randomSeedSeq (engine.cc:756-757),
     // Robot::reset draws one seed per sensor type (robot.cc:137-144; fixed type order Imu, Force, Encoder, Effort, Contact here,
     // the reference iterates an unordered_map), resetAll expands it with a seed_seq into one seed per sensor
@@ -1046,6 +1068,194 @@ static int prepare_sensor_pipeline(JbBatch* b, const uint8_t* mask, bool rows_if
     } else CU(cudaMemcpyAsync(b->d_sp_rng_init, init.data(), sizeof(unsigned long long) * init.size(), cudaMemcpyHostToDevice, b->stream));
     CU(cudaStreamSynchronize(b->stream));
     if (!mask) b->sp_rows_dirty = false;
+    return JB_OK;
+}
+
+int jb_enable_per_env_sensor_options(JbBatch* b, double delay_bound) {
+    if (!b) return fail(JB_ERR_INVALID_ARGUMENT, "null argument");
+    if (b->any_started) return fail(JB_ERR_BAD_CONTROL_FLOW, "Robot already locked, probably because a simulation is running. Please stop it before setting sensor options.");
+    if (!(b->kp.opt.sensors_update_period > 2.3e-16))
+        return fail(JB_ERR_NOT_IMPLEMENTED, "the device measurement pipeline needs a discrete sensorsUpdatePeriod (the delay buffer is sized from it)");
+    if (!(delay_bound >= 0.0) || !std::isfinite(delay_bound)) return fail(JB_ERR_INVALID_ARGUMENT, "delay_bound must be finite and >= 0");
+    CU(cudaSetDevice(b->device));
+    const int counts[5] = {b->kp.nimu, b->kp.nforce, b->kp.nenc, b->kp.neff, b->kp.ncs};
+    const int offs[5] = {b->kp.lay.imu_offset, b->kp.lay.force_offset, b->kp.lay.encoder_offset, b->kp.lay.effort_offset, b->kp.lay.contact_offset};
+    // every sensor in the pipeline, noise and bias on (zero until a row is set), order 1; the values come from the rows
+    b->sdesc.clear();
+    for (int ty = 0; ty < 5; ++ty)
+        for (int k = 0; k < counts[ty]; ++k) {
+            SensorDesc d{};
+            d.type = ty; d.index = k; d.nf = kSensorFields[ty]; d.ns = counts[ty]; d.offset = offs[ty]; d.order = 1;
+            d.has_noise = 1; d.has_bias = 1;
+            b->sdesc.push_back(d);
+        }
+    if (b->sdesc.empty()) return fail(JB_ERR_INVALID_ARGUMENT, "the robot has no sensor");
+    const int ns = static_cast<int>(b->sdesc.size());
+    const int stride = 2 * (b->width + ns) + 5;
+    const size_t rows = static_cast<size_t>(b->n_env) * stride;
+    if (!b->d_sp_env_pending) {
+        int rc;
+        if ((rc = dev_alloc(b, &b->d_sp_env_pending, rows))) return rc;
+        if ((rc = dev_alloc(b, &b->d_sp_env_opt, rows))) return rc;
+        if ((rc = dev_alloc(b, &b->d_sp_env_stage, static_cast<size_t>(b->n_env) * 2 * (b->width + ns)))) return rc;
+        if ((rc = dev_alloc(b, &b->d_sp_env_bad, b->n_env))) return rc;
+    } else {
+        CU(cudaMemsetAsync(b->d_sp_env_pending, 0, rows * sizeof(double), b->stream));
+        CU(cudaMemsetAsync(b->d_sp_env_opt, 0, rows * sizeof(double), b->stream));
+        CU(cudaMemsetAsync(b->d_sp_env_bad, 0, b->n_env * sizeof(int32_t), b->stream));
+    }
+    b->sp_env = true;
+    b->sp_env_bound = delay_bound;
+    b->sp_dirty = true;
+    b->sp_rows_dirty = true;
+    int rc = build_sensor_tables(b);
+    if (rc) return rc;
+    KParams& kp = b->kp;
+    kp.sp_env_on = 1; kp.sp_env_stride = stride;
+    kp.sp_env_pending = b->d_sp_env_pending; kp.sp_env_opt = b->d_sp_env_opt; kp.sp_env_bad = b->d_sp_env_bad;
+    CU(cudaStreamSynchronize(b->stream));
+    return JB_OK;
+}
+
+// Masked rows of the per-env option tables, one thread per env.  A row with a NaN, a negative delay or jitter, or
+// delay + jitter beyond the bound is not written and flags its env (its next start refuses it); a valid row clears the flag.
+__global__ void set_sensor_rows_kernel(double* __restrict__ pending, int32_t* __restrict__ bad_flag, const uint8_t* __restrict__ mask,
+                                       const double* __restrict__ noise, const double* __restrict__ bias, const double* __restrict__ delay,
+                                       const double* __restrict__ jitter, int n_env, int width, int ns, int stride, double bound) {
+    const int e = blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= n_env || (mask && !mask[e])) return;
+    const double* nz = noise + static_cast<size_t>(e) * width;
+    const double* bs = bias + static_cast<size_t>(e) * width;
+    const double* dl = delay + static_cast<size_t>(e) * ns;
+    const double* jt = jitter + static_cast<size_t>(e) * ns;
+    bool bad = false;
+    for (int k = 0; k < width; ++k) bad = bad || !(nz[k] == nz[k]) || !(bs[k] == bs[k]);
+    for (int s = 0; s < ns; ++s) bad = bad || !(dl[s] >= 0.0) || !(jt[s] >= 0.0) || !(dl[s] + jt[s] <= bound);
+    bad_flag[e] = bad ? 1 : 0;
+    if (bad) return;
+    double* row = pending + static_cast<size_t>(e) * stride;
+    for (int k = 0; k < width; ++k) { row[k] = nz[k]; row[width + k] = bs[k]; }
+    for (int s = 0; s < ns; ++s) { row[2 * width + s] = dl[s]; row[2 * width + ns + s] = jt[s]; }
+}
+
+static int launch_sensor_rows(JbBatch* b, const uint8_t* mask_dev, const double* noise, const double* bias, const double* delay,
+                              const double* jitter) {
+    JB_LAUNCH(set_sensor_rows_kernel, static_cast<unsigned>((b->n_env + 127) / 128), 128, 0, b->stream, b->d_sp_env_pending,
+              b->d_sp_env_bad, mask_dev, noise, bias, delay, jitter, b->n_env, b->width, static_cast<int>(b->sdesc.size()),
+              b->kp.sp_env_stride, b->sp_env_bound);
+    CU(cudaGetLastError());
+    ++b->launches;
+    return JB_OK;
+}
+
+int jb_set_sensor_options_env(JbBatch* b, const uint8_t* mask, const double* noise_std, const double* bias, const double* delay,
+                              const double* jitter) {
+    if (!b || !noise_std || !bias || !delay || !jitter) return fail(JB_ERR_INVALID_ARGUMENT, "null argument");
+    if (!b->sp_env) return fail(JB_ERR_BAD_CONTROL_FLOW, "per-env sensor options are not enabled (jb_enable_per_env_sensor_options)");
+    CU(cudaSetDevice(b->device));
+    const int w = b->width, ns = static_cast<int>(b->sdesc.size());
+    for (int e = 0; e < b->n_env; ++e) {
+        if (mask && !mask[e]) continue;
+        for (int k = 0; k < w; ++k) {
+            const double x = noise_std[static_cast<size_t>(e) * w + k], y = bias[static_cast<size_t>(e) * w + k];
+            if (!(x == x) || !(y == y)) return fail(JB_ERR_INVALID_ARGUMENT, "sensor noise_std / bias contains NaN (env " + std::to_string(e) + ").");
+        }
+        for (int s = 0; s < ns; ++s) {
+            const double d = delay[static_cast<size_t>(e) * ns + s], j = jitter[static_cast<size_t>(e) * ns + s];
+            if (!(d >= 0.0) || !(j >= 0.0)) return fail(JB_ERR_INVALID_ARGUMENT, "sensor delay and jitter must be positive (env " + std::to_string(e) + ").");
+            if (!(d + j <= b->sp_env_bound))
+                return fail(JB_ERR_INVALID_ARGUMENT, "sensor delay + jitter exceeds the bound given to jb_enable_per_env_sensor_options (env " + std::to_string(e) + ").");
+        }
+    }
+    double* st = b->d_sp_env_stage;
+    const size_t nw = static_cast<size_t>(b->n_env) * w, nn = static_cast<size_t>(b->n_env) * ns;
+    CU(cudaMemcpyAsync(st, noise_std, nw * sizeof(double), cudaMemcpyHostToDevice, b->stream));
+    CU(cudaMemcpyAsync(st + nw, bias, nw * sizeof(double), cudaMemcpyHostToDevice, b->stream));
+    CU(cudaMemcpyAsync(st + 2 * nw, delay, nn * sizeof(double), cudaMemcpyHostToDevice, b->stream));
+    CU(cudaMemcpyAsync(st + 2 * nw + nn, jitter, nn * sizeof(double), cudaMemcpyHostToDevice, b->stream));
+    if (mask) CU(cudaMemcpyAsync(b->d_mask, mask, b->n_env, cudaMemcpyHostToDevice, b->stream));
+    int rc = launch_sensor_rows(b, mask ? b->d_mask : nullptr, st, st + nw, st + 2 * nw, st + 2 * nw + nn);
+    if (rc) return rc;
+    CU(cudaStreamSynchronize(b->stream));
+    return JB_OK;
+}
+
+int jb_set_sensor_options_env_device(JbBatch* b, const uint8_t* mask_dev, const double* noise_std_dev, const double* bias_dev,
+                                     const double* delay_dev, const double* jitter_dev) {
+    if (!b || !noise_std_dev || !bias_dev || !delay_dev || !jitter_dev) return fail(JB_ERR_INVALID_ARGUMENT, "null argument");
+    if (!b->sp_env) return fail(JB_ERR_BAD_CONTROL_FLOW, "per-env sensor options are not enabled (jb_enable_per_env_sensor_options)");
+    CU(cudaSetDevice(b->device));
+    return launch_sensor_rows(b, mask_dev, noise_std_dev, bias_dev, delay_dev, jitter_dev);
+}
+
+// std::seed_seq{v}.generate(out, out + n) as libstdc++ computes it (bits/random.tcc), 32-bit words held in T
+extern "C++" template <typename T>
+__host__ __device__ inline void seed_seq1_generate(uint32_t v, T* out, int n) {
+    if (n <= 0) return;
+    for (int i = 0; i < n; ++i) out[i] = 0x8b8b8b8bu;
+    const int s = 1;
+    const int t = (n >= 623) ? 11 : (n >= 68) ? 7 : (n >= 39) ? 5 : (n >= 7) ? 3 : (n - 1) / 2;
+    const int p = (n - t) / 2, q = p + t, m = (s + 1 > n) ? s + 1 : n;
+    auto at = [&](int i) { return static_cast<uint32_t>(out[i]); };
+    {
+        const uint32_t r1 = 1371501266u, r2 = r1 + static_cast<uint32_t>(s);
+        out[p] = at(p) + r1;
+        out[q] = at(q) + r2;
+        out[0] = r2;
+    }
+    for (int k = 1; k < m; ++k) {
+        const int kn = k % n, kpn = (k + p) % n, kqn = (k + q) % n;
+        const uint32_t arg = at(kn) ^ at(kpn) ^ at((k - 1) % n);
+        const uint32_t r1 = 1664525u * (arg ^ (arg >> 27));
+        const uint32_t r2 = r1 + static_cast<uint32_t>(kn) + (k <= s ? v : 0u);
+        out[kpn] = at(kpn) + r1;
+        out[kqn] = at(kqn) + r2;
+        out[kn] = r2;
+    }
+    for (int k = m; k < m + n; ++k) {
+        const int kn = k % n, kpn = (k + p) % n, kqn = (k + q) % n;
+        const uint32_t arg = at(kn) + at(kpn) + at((k - 1) % n);
+        const uint32_t r3 = 1566083941u * (arg ^ (arg >> 27));
+        const uint32_t r4 = r3 - static_cast<uint32_t>(kn);
+        out[kpn] = at(kpn) ^ r3;
+        out[kqn] = at(kqn) ^ r4;
+        out[kn] = r4;
+    }
+}
+
+// The seeding chain of prepare_sensor_pipeline for the masked envs, one thread per env
+__global__ void set_seeds_kernel(unsigned long long* __restrict__ rng_init, const uint8_t* __restrict__ mask, const uint32_t* __restrict__ seeds,
+                                 int n_env, int ns, int c0, int c1, int c2, int c3, int c4) {
+    const int e = blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= n_env || (mask && !mask[e])) return;
+    const int counts[5] = {c0, c1, c2, c3, c4};
+    uint32_t buf[2];
+    seed_seq1_generate(seeds[e], buf, 2);
+    unsigned long long st = (static_cast<unsigned long long>(buf[0]) | (static_cast<unsigned long long>(buf[1]) << 32)) | 3ULL;
+    unsigned long long* row = rng_init + static_cast<size_t>(e) * ns;
+    for (int ty = 0; ty < 5; ++ty) {
+        if (!counts[ty]) continue;
+        seed_seq1_generate(pcg32_next(st), row, counts[ty]);
+        for (int k = 0; k < counts[ty]; ++k) row[k] |= 3ULL;
+        row += counts[ty];
+    }
+}
+
+int jb_set_seeds_device(JbBatch* b, const uint8_t* mask_dev, const uint32_t* seeds_dev) {
+    if (!b || !seeds_dev) return fail(JB_ERR_INVALID_ARGUMENT, "null argument");
+    if (b->sdesc.empty()) return fail(JB_ERR_BAD_CONTROL_FLOW, "no sensor has options: the measurement pipeline is off, there is nothing to seed");
+    CU(cudaSetDevice(b->device));
+    // the envs outside the mask keep the start states of their host seeds: upload those first if they are not on the device
+    if (!b->sp_seeds_dev) {
+        int rc = prepare_sensor_pipeline(b, nullptr, true);
+        if (rc) return rc;
+    }
+    const KParams& kp = b->kp;
+    JB_LAUNCH(set_seeds_kernel, static_cast<unsigned>((b->n_env + 127) / 128), 128, 0, b->stream, b->d_sp_rng_init, mask_dev, seeds_dev,
+              b->n_env, kp.sp_nsens, kp.nimu, kp.nforce, kp.nenc, kp.neff, kp.ncs);
+    CU(cudaGetLastError());
+    ++b->launches;
+    b->sp_seeds_dev = true;
     return JB_OK;
 }
 

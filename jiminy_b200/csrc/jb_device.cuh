@@ -179,6 +179,13 @@ struct KParams {
     // force-carrying hot path (env_step_kernel_ext): copies of the latched profile / process values taken at the top of the
     // pass, [MAX_PROFILE + MAX_PROCESS][6][n_pad] (restored on hand-off)
     double* latch_snap;
+    // per-env sensor options (jb_enable_per_env_sensor_options), read only by write_sensors / measure_sensor.  One row of
+    // sp_env_stride doubles per env: noise_std [width] | bias [width] (columns of the sensor matrix) | delay [sp_nsens] |
+    // jitter [sp_nsens] (pipeline order) | delayMax [5] (per sensor type, computed when the row is latched)
+    int32_t sp_env_on, sp_env_stride;
+    const double* sp_env_pending;  // [n_env][stride] rows written by the setters
+    double* sp_env_opt;            // [n_env][stride] rows latched at the env's last start
+    int32_t* sp_env_bad;           // [n_env] 1: the last device row was rejected, the env's next start refuses it
 };
 
 // Launch parameters live in constant memory (uniform constant-bank operands in every device
@@ -3022,10 +3029,12 @@ JB_DI int sensor_ring_push(int env, double t) {
     int32_t* cnt = KP->sp_count + static_cast<size_t>(env) * 6;
     double* tm = KP->sp_times + static_cast<size_t>(env) * cap;
     const int head = (cnt[0] + 1) % cap;
+    const double* dmax = KP->sp_env_on ? KP->sp_env_opt + static_cast<size_t>(env) * KP->sp_env_stride + 2 * (KP->lay.width + KP->sp_nsens)
+                                       : KP->sp_delay_max;
     for (int ty = 0; ty < 5; ++ty) {
         const int n = cnt[1 + ty];
         const double front = tm[((head - 1 - (n - 1)) % cap + cap) % cap];      // oldest sample this type still holds
-        const double timeMin = t - KP->sp_delay_max[ty] - 0.02;                 // SIMULATION_MAX_TIMESTEP
+        const double timeMin = t - dmax[ty] - 0.02;                             // SIMULATION_MAX_TIMESTEP
         // rotate (drop the oldest) or grow; a full buffer always drops (older than anything a lookup can reach)
         if (!(timeMin > front) && n < cap) cnt[1 + ty] = n + 1;
     }
@@ -3044,8 +3053,21 @@ JB_DI void measure_sensor(int env, int s) {
     const int head = cnt[0], n = cnt[1 + d->type];
     unsigned long long st = KP->sp_rng[static_cast<size_t>(env) * KP->sp_nsens + s];
     auto phys = [&](int i) { return ((head - (n - 1) + i) % cap + cap) % cap; };   // logical index (0 = oldest of this type) -> slot
-    const float jit = static_cast<float>(d->jitter);
-    const double delay = d->delay + static_cast<double>((jit - 0.0f) * rng_uniform01(st) + 0.0f);
+    // options: the batch-wide descriptor, or this env's latched row (noise and bias at the sensor's own columns, field
+    // stride d->ns like the measurement row; noise and bias always on)
+    double d_delay = d->delay, d_jitter = d->jitter;
+    const double *nstd = d->noise_std, *bias = d->bias;
+    int fstride = 1;
+    if (KP->sp_env_on) {
+        const double* o = KP->sp_env_opt + static_cast<size_t>(env) * KP->sp_env_stride;
+        nstd = o + d->offset + d->index;
+        bias = nstd + width;
+        fstride = d->ns;
+        d_delay = o[2 * width + s];
+        d_jitter = o[2 * width + KP->sp_nsens + s];
+    }
+    const float jit = static_cast<float>(d_jitter);
+    const double delay = d_delay + static_cast<double>((jit - 0.0f) * rng_uniform01(st) + 0.0f);
     double timeDesired = tm[head] - delay;
     if (d->order == 0) timeDesired += STEPPER_MIN_TIMESTEP;
     int idxLeft;
@@ -3069,7 +3091,7 @@ JB_DI void measure_sensor(int env, int s) {
         i0 = idxLeft < 0 ? 0 : idxLeft;        // (idxLeft < 0: "No data old enough" in the reference; the buffer is sized so that it cannot happen)
         if (d->order == 0) mode = 0;
         else { mode = 1; i1 = i0 + 1; ratio = (timeDesired - tm[phys(i0)]) / (tm[phys(i1)] - tm[phys(i0)]); }
-    } else if (d->delay > D_EPS || d->jitter > D_EPS) {
+    } else if (d_delay > D_EPS || d_jitter > D_EPS) {
         // the buffer is not old enough yet: the oldest value that is not the initial zero sample
         i0 = n - 1;
         for (int i = 0; i < n; ++i) if (tm[phys(i)] > 0.0) { i0 = i - 1 < 0 ? 0 : i - 1; break; }
@@ -3080,11 +3102,11 @@ JB_DI void measure_sensor(int env, int s) {
     for (int f = 0; f < d->nf; ++f) {
         const double a = r0[f * d->ns];
         double val = mode == 1 ? a + ratio * (r1[f * d->ns] - a) : a;
-        if (d->has_noise) val += static_cast<double>(rng_normal(st) * static_cast<float>(d->noise_std[f]) + 0.0F);
+        if (d->has_noise) val += static_cast<double>(rng_normal(st) * static_cast<float>(nstd[f * fstride]) + 0.0F);
         out[d->offset + f * d->ns + d->index] = val;
     }
     if (d->has_bias)
-        for (int f = 0; f < d->nf; ++f) out[d->offset + f * d->ns + d->index] += d->bias[f];
+        for (int f = 0; f < d->nf; ++f) out[d->offset + f * d->ns + d->index] += bias[f * fstride];
     KP->sp_rng[static_cast<size_t>(env) * KP->sp_nsens + s] = st;
 }
 
@@ -3126,6 +3148,23 @@ __device__ __noinline__ void write_sensors(const Ctx c, const bool at_start, con
     const JbSensorLayout& lay = KP->lay;
     double* row = KP->sensors + static_cast<size_t>(c.env) * lay.width;
     if (KP->sp_on) {
+        if (at_start && KP->sp_env_on) {
+            // per-env options: the row last written for this env becomes the one its episode runs with (setOptions
+            // before Engine::reset in the reference), and its per-type delayMax follows (abstract_sensor.hxx:199-232)
+            const size_t o = static_cast<size_t>(c.env) * KP->sp_env_stride;
+            const int nrow = 2 * (lay.width + KP->sp_nsens);
+            for (int k = c.sub; k < nrow; k += L) KP->sp_env_opt[o + k] = KP->sp_env_pending[o + k];
+            if (c.sub == 0) {
+                const double* pd = KP->sp_env_pending + o + 2 * lay.width;
+                double* dmax = KP->sp_env_opt + o + nrow;
+                for (int ty = 0; ty < 5; ++ty) dmax[ty] = 0.0;
+                for (int s = 0; s < KP->sp_nsens; ++s) {
+                    const int ty = KP->sp_desc[s].type;
+                    dmax[ty] = fmax(dmax[ty], pd[s] + pd[KP->sp_nsens + s]);
+                }
+            }
+            jb_syncwarp(c);
+        }
         // measurement pipeline: the true values go to a new slot of the env's ring, the public row receives the measurements
         if (c.sub == 0) {
             if (at_start) {

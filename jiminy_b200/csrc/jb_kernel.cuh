@@ -405,6 +405,11 @@ __device__ __forceinline__ void env_step_body(const LaunchArgs& la, const bool o
                 return;
             }
         }
+        // per-env sensor options: the last row jb_set_sensor_options_env_device received for this env was rejected
+        if (mode == MODE_START && KP->sp_env_on && KP->sp_env_bad[c.env] != 0) {
+            if (c.valid && c.sub == 0) KP->status[c.env] = JB_ENV_NOT_STARTED | JB_ENV_BAD_START;
+            return;
+        }
     }
     if (mode == MODE_STEP && (status & (JB_ENV_NOT_STARTED | JB_ENV_NAN | JB_ENV_ITER_FAILED | JB_ENV_DT_UNDERFLOW | JB_ENV_SOLVER_FAILED))) {
         JB_EMUL_LEAVES_EARLY(FAST ? 0 : 1);

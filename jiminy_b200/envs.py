@@ -21,7 +21,7 @@ from typing import Any, Dict, Optional, Tuple
 
 import numpy as np
 
-from . import core, scenarios
+from . import core, scenarios, sensor_randomisation
 from .disturbance import from_std_ratio
 from .model import RobotTable
 
@@ -103,8 +103,9 @@ def configure_pd_blocks(env, kp, kd, joint_position_margin: float, joint_velocit
 class BatchedJiminyEnv:
     def __init__(self, scenario: scenarios.Scenario, device: int = 0, height_threshold_ratio: float = 0.5,
                  simulation_duration_max: float = 20.0, api_: Optional[core.Api] = None, std_ratio: Optional[dict] = None):
-        """`std_ratio`: the reference walker env's randomisation ratios.  None or {}: none; {"disturbance": r}: the walker
-        disturbance forces (`jiminy_b200.disturbance`), re-drawn for every env that (re)starts."""
+        """`std_ratio`: the reference walker env's randomisation ratios.  None or {}: none; "disturbance": r, the walker
+        disturbance forces (`jiminy_b200.disturbance`); "sensors": r, noise, bias, delay and jitter of every sensor and a
+        new seed of its generators (`jiminy_b200.sensor_randomisation`).  Both are re-drawn for every env that (re)starts."""
         self.sc = scenario
         self.robot: RobotTable = scenario.robot
         self.n_env, self.step_dt = scenario.n_env, scenario.step_dt
@@ -128,6 +129,11 @@ class BatchedJiminyEnv:
         if self.disturbance is not None:
             self.disturbance.register(self.engine)
             self._disturbance_rng = np.random.default_rng([scenario.seed, 0xD157])
+        self.sensor_randomisation = sensor_randomisation.from_std_ratio(self.robot.sensor_layout(), std_ratio)
+        if self.sensor_randomisation is not None:
+            self.sensor_randomisation.register(self.engine)
+            self._sensor_rng = np.random.default_rng([scenario.seed, 0x5E45])
+            self.sensor_rows: Optional[Dict[str, np.ndarray]] = None      # the options and seed every env runs with
         self._started = False
 
     # ------------------------------------------------------------------ helpers
@@ -153,18 +159,30 @@ class BatchedJiminyEnv:
             draw = self.disturbance.draw_numpy(self._disturbance_rng, self.n_env)
             self.disturbance.apply_host(self.engine, draw, mask)
 
+    def _redraw_sensors(self, mask: Optional[np.ndarray]) -> None:
+        """New sensor options and seeds for the envs about to (re)start (`_setup`, locomotion.py:264-286)."""
+        if self.sensor_randomisation is not None:
+            draw = self.sensor_randomisation.draw_numpy(self._sensor_rng, self.n_env)
+            if mask is not None and self.sensor_rows is not None:
+                sel = np.asarray(mask).astype(bool)
+                draw = {k: np.where(sel.reshape((-1,) + (1,) * (v.ndim - 1)), v, self.sensor_rows[k]) for k, v in draw.items()}
+            self.sensor_rows = draw
+            self.sensor_randomisation.apply_host(self.engine, draw, mask)
+
     # ------------------------------------------------------------------ gym API
     def reset(self, mask: Optional[np.ndarray] = None) -> Tuple[Dict[str, Any], Dict[str, Any]]:
         if mask is None or not self._started:
             q0, v0 = (self.sc.q0, self.sc.v0) if not self._started else self._sample_state(self.n_env)
             self.engine.set_command(self.sc.target0)
             self._redraw_disturbance(None)
+            self._redraw_sensors(None)
             self.engine.start(q0, v0)
             self.num_steps[:] = 0
             self._started = True
         elif mask.any():
             q0, v0 = self._sample_state(self.n_env)
             self._redraw_disturbance(mask)
+            self._redraw_sensors(mask)
             self.engine.start(q0, v0, mask=mask)
             self.num_steps[mask.astype(bool)] = 0
         return self._observation(), {}
@@ -232,6 +250,7 @@ class PDControlBatchedEnv(BatchedJiminyEnv):
             self.engine.set_command(np.zeros((self.n_env, self.robot.nmotors)))
             q0, v0 = (self.sc.q0, self.sc.v0) if not self._started else self._sample_state(self.n_env)
             self._redraw_disturbance(None)
+            self._redraw_sensors(None)
             self.engine.start(q0, v0)
             self.num_steps[:] = 0
             self._started = True

@@ -26,6 +26,12 @@ impulse setter's checks (NaN, t < 0, dt < 1e-10) flag a rejected row's env NOT_S
 enqueued right after it clears that flag and the env runs on with its previous impulse row: the sampler never draws such a
 row (t >= 1.75 s, dt = 10 ms, finite wrenches), so nothing here depends on the flag.
 
+Sensors.  With `std_ratio={"sensors": r}` the sensor options (noise, bias, delay, jitter) and engine seeds of the envs in
+the done mask are re-drawn the same way (`jiminy_b200.sensor_randomisation`) and written by
+`jb_set_sensor_options_env_device` and `jb_set_seeds_device` before the masked restart, which latches them.
+`env.sensor_rows` holds the options and seed every env currently runs with.  The sampler never draws a row the setter
+would reject (its delays stay below the bound the buffer was sized for).
+
 Streams.  All work runs on the batch's own stream (`torch.cuda.ExternalStream(engine.stream())`).  On entry it waits
 for the caller's current stream; on exit the caller's current stream waits for it.  With the CPU emulation of the
 library (`api_` given), device memory is host memory: the env then runs on `torch_device="cpu"`, without streams.
@@ -100,6 +106,11 @@ class DeviceBatchedEnv(envs.BatchedJiminyEnv):
             self._disturbance_gen.manual_seed(int(np.random.default_rng([self.sc.seed, 0xD157]).integers(0, 2 ** 31 - 1)))
             with self._on_batch_stream():     # the draw's first use of its kernels on the batch stream happens here
                 self.disturbance_rows = self.disturbance.draw_torch(self._disturbance_gen, n, dev)
+        if self.sensor_randomisation is not None:
+            self._sensor_gen = torch.Generator(device=dev)
+            self._sensor_gen.manual_seed(int(np.random.default_rng([self.sc.seed, 0x5E45]).integers(0, 2 ** 31 - 1)))
+            with self._on_batch_stream():
+                self.sensor_rows = self.sensor_randomisation.draw_torch(self._sensor_gen, n, dev)
         self.num_steps = torch.zeros(n, dtype=torch.int64, device=dev)
         # zero-copy views of the batch's device buffers
         ptr = eng.device_state_ptrs()
@@ -187,6 +198,17 @@ class DeviceBatchedEnv(envs.BatchedJiminyEnv):
                 rows[k].copy_(torch.where(done.view(-1, 1), new[k], rows[k]))
         self.disturbance.apply_device(self.engine, rows, None if done is None else self._mask.data_ptr())
 
+    def _redraw_sensors(self, done: Optional[torch.Tensor]) -> None:
+        """New sensor options and seeds for the envs of `done` (None: all), drawn on the device and written by the device
+        setters with the mask in `self._mask`; `sensor_rows` keeps what every env runs with."""
+        if self.sensor_randomisation is None:
+            return
+        new = self.sensor_randomisation.draw_torch(self._sensor_gen, self.n_env, self.torch_device)
+        rows = self.sensor_rows
+        for k in rows:
+            rows[k].copy_(new[k] if done is None else torch.where(done.view(-1, *([1] * (rows[k].dim() - 1))), new[k], rows[k]))
+        self.sensor_randomisation.apply_device(self.engine, rows, None if done is None else self._mask.data_ptr())
+
     def _restart(self, done: torch.Tensor) -> torch.Tensor:
         """Masked restart of the envs in `done` from bank rows drawn on the device; returns the rows (-1: not restarted)."""
         q_bank, v_bank = self.reset_states
@@ -195,6 +217,7 @@ class DeviceBatchedEnv(envs.BatchedJiminyEnv):
         torch.index_select(v_bank, 0, rows, out=self._v_start)
         self._mask.copy_(done)
         self._redraw_disturbance(done)
+        self._redraw_sensors(done)
         self.engine.start_device(self._q_start.data_ptr(), self._v_start.data_ptr(), self._mask.data_ptr())
         self.num_steps.masked_fill_(done, 0)
         return torch.where(done, rows, torch.full_like(rows, -1))
@@ -208,6 +231,7 @@ class DeviceBatchedEnv(envs.BatchedJiminyEnv):
             if not self._started:
                 self._first_command()
                 self._redraw_disturbance(None)
+                self._redraw_sensors(None)
                 self.engine.start(self.sc.q0, self.sc.v0)
                 self.num_steps.zero_()
                 self._started = True

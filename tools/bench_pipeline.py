@@ -21,8 +21,12 @@ time, none within the default `--duration-max`, and the profile evaluated at eve
 restart) and runs each loop with it off and on, alternating in one process, `max(--alternate, 1)` rounds.  On ANYmal the
 forces ride the quadruped hot path (`env_step_kernel_ext`); Atlas runs the generic kernel either way.
 
+`--sensors R` does the same for the walker sensor randomisation (`std_ratio={"sensors": R}`: per-env noise, bias, delay
+and jitter of every sensor and fresh generator seeds, re-drawn at every restart); with both options both are on in the
+"on" runs.
+
     python tools/bench_pipeline.py [--robot atlas|anymal] [--loop host|device] [--alternate R] [--n-env 4096]
-                                   [--steps 10] [--warmup 3] [--duration-max 0.4] [--disturbance R]
+                                   [--steps 10] [--warmup 3] [--duration-max 0.4] [--disturbance R] [--sensors R]
 """
 import argparse
 import json
@@ -42,9 +46,10 @@ KEYS = [("states", "pd_controller"), ("measurements", "EncoderSensor"), ("featur
 
 
 def make_env(n_env: int, api_=None, robot: str = "atlas", loop: str = "host", duration_max: float = 20.0,
-             disturbance: float = 0.0):
+             disturbance: float = 0.0, sensors: float = 0.0):
     from jiminy_b200 import envs, scenarios
-    kw = dict(simulation_duration_max=duration_max, api_=api_, std_ratio={"disturbance": disturbance} if disturbance > 0 else None)
+    ratio = {k: r for k, r in (("disturbance", disturbance), ("sensors", sensors)) if r > 0}
+    kw = dict(simulation_duration_max=duration_max, api_=api_, std_ratio=ratio or None)
     if robot == "anymal":
         from jiminy_b200.torch_envs import DeviceBatchedEnv
         return (DeviceBatchedEnv if loop == "device" else envs.BatchedJiminyEnv)(scenarios.make("anymal", n_env, seed=0), **kw)
@@ -77,10 +82,10 @@ def gpu_info() -> dict:
 
 
 def run(n_env: int, steps: int, warmup: int, api_=None, robot: str = "atlas", loop: str = "host",
-        duration_max: float = 0.4, disturbance: float = 0.0) -> dict:
+        duration_max: float = 0.4, disturbance: float = 0.0, sensors: float = 0.0) -> dict:
     import torch
     from jiminy_b200.envs import flatten_observation
-    env = make_env(n_env, api_, robot, loop, duration_max, disturbance)
+    env = make_env(n_env, api_, robot, loop, duration_max, disturbance, sensors)
     device = loop == "device"
     on_gpu = device and env.torch_device.type == "cuda"
     nm = env.robot.nmotors
@@ -123,7 +128,7 @@ def run(n_env: int, steps: int, warmup: int, api_=None, robot: str = "atlas", lo
             f"contacts, euler_explicit 5 ms" if robot == "atlas" else
             "anymal PD standing (plain PD law), spring-damper contacts, runge_kutta_4 1 ms, per-step position targets")
     out = {"metric": "env_steps_per_sec", "unit": "env-steps/s", "value": n_env * steps / dt, "ms_per_step": 1e3 * dt / steps,
-           "loop": loop, "robot": robot, "disturbance": disturbance, "n_env": n_env, "steps": steps, "warmup": warmup,
+           "loop": loop, "robot": robot, "disturbance": disturbance, "sensors": sensors, "n_env": n_env, "steps": steps, "warmup": warmup,
            "timing": "host clock around env.step + flatten_observation, ending in a device synchronise",
            "config": {"workload": f"{desc}, {n_env} envs, step_dt {env.step_dt}, simulation_duration_max {duration_max}",
                       "env": type(env).__name__, "lane_plan": env.engine.describe(), "observation_width": int(flat.shape[1])},
@@ -152,22 +157,24 @@ def alternate(rounds: int, **kw) -> dict:
     return out
 
 
-def alternate_disturbance(rounds: int, ratio: float, loops, **kw) -> dict:
-    """Each loop with the disturbance off and on, `rounds` times in this process, alternating; env-steps/s and spread."""
-    runs = {(loop, r): [] for loop in loops for r in (0.0, ratio)}
+def alternate_randomisation(rounds: int, ratios: dict, loops, **kw) -> dict:
+    """Each loop with the randomisation of `ratios` ({"disturbance": r} and / or {"sensors": r}) off and on, `rounds`
+    times in this process, alternating; env-steps/s and spread."""
+    name = "_".join(ratios)
+    runs = {(loop, on): [] for loop in loops for on in (False, True)}
     for _ in range(rounds):
         for loop in loops:
-            for r in (0.0, ratio):
-                runs[(loop, r)].append(run(loop=loop, disturbance=r, **kw))
+            for on in (False, True):
+                runs[(loop, on)].append(run(loop=loop, **(ratios if on else {}), **kw))
     out = {"metric": "env_steps_per_sec", "unit": "env-steps/s", "robot": kw.get("robot", "atlas"), "rounds": rounds}
-    for (loop, r), rs in runs.items():
+    for (loop, on), rs in runs.items():
         v = sorted(x["value"] for x in rs)
-        out[f"{loop}_disturbance_{'on' if r > 0 else 'off'}"] = {
+        out[f"{loop}_{name}_{'on' if on else 'off'}"] = {
             "median": float(np.median(v)), "min": v[0], "max": v[-1], "ms_per_step_median": float(np.median([x["ms_per_step"] for x in rs])),
             "envs_restarted": [x["envs_restarted"] for x in rs], "envs_flagged": [x["envs_flagged"] for x in rs],
             "config": rs[-1]["config"]}
     for loop in loops:
-        out[f"{loop}_on_over_off_median"] = out[f"{loop}_disturbance_on"]["median"] / out[f"{loop}_disturbance_off"]["median"]
+        out[f"{loop}_on_over_off_median"] = out[f"{loop}_{name}_on"]["median"] / out[f"{loop}_{name}_off"]["median"]
     return out
 
 
@@ -181,10 +188,12 @@ if __name__ == "__main__":
     ap.add_argument("--alternate", type=int, default=0, metavar="R")
     ap.add_argument("--duration-max", type=float, default=0.4)
     ap.add_argument("--disturbance", type=float, default=0.0, metavar="R")
+    ap.add_argument("--sensors", type=float, default=0.0, metavar="R")
     a = ap.parse_args()
     kw = dict(n_env=a.n_env, steps=a.steps, warmup=a.warmup, robot=a.robot, duration_max=a.duration_max)
-    if a.disturbance > 0:
-        res = alternate_disturbance(max(a.alternate, 1), a.disturbance, ("host", "device") if a.alternate > 0 else (a.loop,), **kw)
+    ratios = {k: r for k, r in (("disturbance", a.disturbance), ("sensors", a.sensors)) if r > 0}
+    if ratios:
+        res = alternate_randomisation(max(a.alternate, 1), ratios, ("host", "device") if a.alternate > 0 else (a.loop,), **kw)
     else:
         res = alternate(a.alternate, **kw) if a.alternate > 0 else run(loop=a.loop, **kw)
     res.update(gpu_info())
