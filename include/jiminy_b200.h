@@ -441,6 +441,28 @@ int jb_device_block_views(JbBatch* batch, int32_t** status, double** pd_state, d
 int jb_set_model_variants(JbBatch* batch, int32_t n_variants, const JbModelDesc* models, const int32_t* variant_of_group);
 int jb_envs_per_group(JbBatch* batch);
 
+/* Per-env flexibility parameters: the walker env's `model` randomisation (gym_jiminy locomotion.py:288-296) re-draws the
+ * stiffness and damping of every flexibility joint at every reset, with envs restarting while others run.
+ * jb_enable_per_env_flexibility gives every env its own row [n_flex][6] (stiffness xyz, then damping xyz of each
+ * flexibility), flexibilities in the order of `flex_joints` [n_flex] -- the joint indices of the model's spherical
+ * joints, each once (`robot.flexibility_joint_indices`); NULL: increasing joint index.  Two device tables, pending and
+ * active, both start from each env's model values (its variant's with jb_set_model_variants).  Refused
+ * (JB_ERR_INVALID_ARGUMENT) on a model without flexibility joints, with a list that is not a permutation of them, and on
+ * a second call.
+ * jb_set_flexibility_env writes the pending rows [n_env][n_flex][6] of the envs selected by mask (NULL = all).  An env
+ * runs with its pending row from its next start (jb_start with the env in its mask, or jb_start_device), which copies it
+ * into the active row before the start's own evaluations; a running env is not affected.  The active rows override the
+ * stiffness and damping of every variant; the variant's other numbers still apply.  A row with a value that is not
+ * finite or is negative (Model::setOptions, model.cc:1620-1626) is refused: the host form writes nothing and returns
+ * JB_ERR_INVALID_ARGUMENT naming the env; the _device form (device buffers, one kernel on the batch stream, no host
+ * synchronisation) skips that row and marks the env, whose starts then leave it JB_ENV_NOT_STARTED | JB_ENV_BAD_START
+ * until a valid row for it is written.  The mark is the flexibility setter's own: sensor rows neither set nor clear it.
+ * jb_get_flexibility_env reads the active rows [n_env][n_flex][6]. */
+int jb_enable_per_env_flexibility(JbBatch* batch, int32_t n_flex, const int32_t* flex_joints);
+int jb_set_flexibility_env(JbBatch* batch, const uint8_t* mask, const double* rows);
+int jb_set_flexibility_env_device(JbBatch* batch, const uint8_t* mask_dev, const double* rows_dev);
+int jb_get_flexibility_env(JbBatch* batch, double* out);
+
 /* Stable zero-copy views of the state, like the `StepperState` / `RobotState` members the reference exposes to Python as
  * array views of the engine's own memory (python/jiminy_pywrap/include/jiminy/python/functors.h:57-68, generic.py:688-690:
  * a gym env reads `q`, `v`, the sensor matrix every step without a getter call).  The first call with `host` non-null

@@ -67,7 +67,9 @@ class Api:
                "jb_start_device", "jb_set_pd_adapter", "jb_pd_adapter_device", "jb_device_block_views",
                "jb_set_impulse_force_device", "jb_register_process_force", "jb_set_process_force",
                "jb_set_process_force_device", "jb_enable_per_env_sensor_options", "jb_set_sensor_options_env",
-               "jb_set_sensor_options_env_device", "jb_set_seeds_device")
+               "jb_set_sensor_options_env_device", "jb_set_seeds_device",
+               "jb_enable_per_env_flexibility", "jb_set_flexibility_env", "jb_set_flexibility_env_device",
+               "jb_get_flexibility_env")
 
     def __init__(self, cdll: C.CDLL):
         self.dll = L = cdll
@@ -143,6 +145,10 @@ class Api:
         L.jb_set_sensor_options_env.argtypes = [vp, c_uint8_p] + [c_double_p] * 4
         L.jb_set_sensor_options_env_device.argtypes = [vp] + [vp] * 5
         L.jb_set_seeds_device.argtypes = [vp, vp, vp]
+        L.jb_enable_per_env_flexibility.argtypes = [vp, C.c_int32, c_int32_p]
+        L.jb_set_flexibility_env.argtypes = [vp, c_uint8_p, c_double_p]
+        L.jb_set_flexibility_env_device.argtypes = [vp, vp, vp]
+        L.jb_get_flexibility_env.argtypes = [vp, c_double_p]
 
     def check(self, rc: int) -> None:
         if rc != JB_OK:
@@ -546,6 +552,37 @@ class BatchedEngine:
         self._api.check(self._api.dll.jb_set_sensor_options_env_device(
             self._h, C.c_void_p(mask_ptr or None), C.c_void_p(noise_std_ptr), C.c_void_p(bias_ptr), C.c_void_p(delay_ptr),
             C.c_void_p(jitter_ptr)))
+
+    # ---- per-env flexibility parameters (the walker env's `model` randomisation)
+    @property
+    def n_flex(self) -> int:
+        """Flexibility joints of the robot: the rows of `set_flexibility_env`, in `robot.flexibility_joint_indices` order."""
+        return len(self.robot.flexibility_joint_names)
+
+    def enable_per_env_flexibility(self) -> None:
+        """Per-env stiffness and damping of every flexibility joint (`set_flexibility_env`), starting from each env's
+        model values.  Refused on a robot without flexibility joints and on a second call."""
+        j = np.ascontiguousarray(self.robot.flexibility_joint_indices, dtype=np.int32)
+        self._api.check(self._api.dll.jb_enable_per_env_flexibility(self._h, len(j), j.ctypes.data_as(c_int32_p)))
+
+    def set_flexibility_env(self, rows, mask: Optional[np.ndarray] = None) -> None:
+        """Rows [n_env, n_flex, 6] (stiffness xyz, damping xyz per flexibility) of the envs of `mask` (None = all), applied
+        from each env's next start.  A value that is not finite or is negative raises ValueError and nothing is written."""
+        rows = self._per_env(rows, (self.n_flex, 6))
+        m = None if mask is None else np.ascontiguousarray(mask, dtype=np.uint8)
+        self._api.check(self._api.dll.jb_set_flexibility_env(self._h, None if m is None else m.ctypes.data_as(c_uint8_p), dptr(rows)))
+
+    def set_flexibility_env_device(self, rows_ptr: int, mask_ptr: Optional[int] = None) -> None:
+        """`set_flexibility_env` from a device buffer of the same layout (fp64; mask [n_env] uint8 or None), enqueued on
+        the batch stream with no host synchronisation.  A rejected row is not written and its env stays
+        JB_ENV_NOT_STARTED | JB_ENV_BAD_START through its starts until a valid row for it arrives."""
+        self._api.check(self._api.dll.jb_set_flexibility_env_device(self._h, C.c_void_p(mask_ptr or None), C.c_void_p(rows_ptr)))
+
+    def get_flexibility_env(self) -> np.ndarray:
+        """The rows every env runs with (latched at its last start), [n_env, n_flex, 6]."""
+        out = np.zeros((self.n_env, self.n_flex, 6))
+        self._api.check(self._api.dll.jb_get_flexibility_env(self._h, dptr(out)))
+        return out
 
     def get_sensor_data(self) -> np.ndarray:
         out = np.zeros((self.n_env, max(self.width, 1)))

@@ -119,6 +119,12 @@ struct JbBatch {
     double* d_proc_stage[MAX_PROCESS] = {};
     size_t proc_tab_cap[MAX_PROCESS] = {}, proc_stage_cap[MAX_PROCESS] = {};   // doubles allocated (kept across jb_remove_all_forces)
     double* d_proc_latched = nullptr;
+    // model variants (jb_set_model_variants): the host copies of the tables and of the variant of every group
+    std::vector<RecDbl> h_variant_rows;
+    std::vector<int32_t> h_variant_of_group;
+    // per-env flexibility parameters (jb_enable_per_env_flexibility): pending / active rows, host-setter staging, reject flags
+    double *d_flex_pending = nullptr, *d_flex_active = nullptr, *d_flex_stage = nullptr;
+    int32_t *d_flex_bad = nullptr, *d_flex_of_rec = nullptr;
 };
 
 // The dynamic shared-memory opt-in is a per-function, per-device attribute: only ever raise it.
@@ -131,6 +137,7 @@ static int raise_smem_attr(int device, size_t bytes) {
     cudaError_t e = cudaFuncSetAttribute(env_step_kernel_t<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(bytes));
     if (e == cudaSuccess) e = cudaFuncSetAttribute(env_step_kernel_t<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(bytes));
     if (e == cudaSuccess) e = cudaFuncSetAttribute(env_step_kernel_ext, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(bytes));
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(env_step_kernel_flex, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(bytes));
     if (e != cudaSuccess) return fail(JB_ERR_CUDA, std::string("cudaFuncSetAttribute: ") + cudaGetErrorString(e));
     g_smem_attr[device] = bytes;
 #endif
@@ -228,15 +235,17 @@ static int launch(JbBatch* b, int mode, double step_dt, const uint8_t* d_mask = 
         la.peer_step = b->step_id;
     }
     // the hot-path kernel hands envs that leave the hot path over to the full body inside the same launch
+    // (per-env flexibility parameters: every launch runs env_step_kernel_flex)
     const bool fast = mode == MODE_STEP && kp.n_eslot == 0 && kp.opt.contact_model == JB_CONTACT_SPRING_DAMPER &&
-                      kp.opt.ode_solver != JB_SOLVER_RUNGE_KUTTA_DOPRI && !b->no_fast_kernel;
+                      kp.opt.ode_solver != JB_SOLVER_RUNGE_KUTTA_DOPRI && !b->no_fast_kernel && !kp.flex_on;
     const bool fast_ext = mode == MODE_STEP && forces_on_hot_path(b);
     const int epw = 32 / b->plan.L;
     const int nblocks = (b->n_env + epw - 1) / epw;
 #ifdef JB_HOST_EMUL
     emul::current_L = b->plan.L;
     g_kp_host = kp;
-    if (fast) JB_LAUNCH(env_step_kernel_t<true>, nblocks, 32, b->smem_bytes, b->stream, la);
+    if (kp.flex_on) JB_LAUNCH(env_step_kernel_flex, nblocks, 32, b->smem_bytes, b->stream, la);
+    else if (fast) JB_LAUNCH(env_step_kernel_t<true>, nblocks, 32, b->smem_bytes, b->stream, la);
     else if (fast_ext) JB_LAUNCH(env_step_kernel_ext, nblocks, 32, b->smem_bytes, b->stream, la);
     else JB_LAUNCH(env_step_kernel_t<false>, nblocks, 32, b->smem_bytes, b->stream, la);
 #else
@@ -253,7 +262,8 @@ static int launch(JbBatch* b, int mode, double step_dt, const uint8_t* d_mask = 
             g_kp_valid[b->device] = true;
             ++b->param_uploads;
         }
-        if (fast) JB_LAUNCH(env_step_kernel_t<true>, nblocks, 32, b->smem_bytes, b->stream, la);
+        if (kp.flex_on) JB_LAUNCH(env_step_kernel_flex, nblocks, 32, b->smem_bytes, b->stream, la);
+        else if (fast) JB_LAUNCH(env_step_kernel_t<true>, nblocks, 32, b->smem_bytes, b->stream, la);
         else if (fast_ext) JB_LAUNCH(env_step_kernel_ext, nblocks, 32, b->smem_bytes, b->stream, la);
         else JB_LAUNCH(env_step_kernel_t<false>, nblocks, 32, b->smem_bytes, b->stream, la);
         CU(cudaEventRecord(evt, b->stream));
@@ -635,6 +645,10 @@ int jb_describe(JbBatch* b, char* buf, int32_t len) {
                   forces_on_hot_path(b) ? ", external forces applied in the evaluation" : "",
                   !b->kp.cons_on ? "flag only" : (b->kp.cq_on ? (b->kp.lb_on ? "structured quadruped solver + lane-block solver" : "structured quadruped solver + generic")
                                                  : (b->kp.bd_on ? "body-space contact solver + lane-block solver" : (b->kp.lb_on ? "lane-block solver" : "generic solver"))));
+    if (b->kp.flex_on) {
+        const size_t used = std::strlen(buf);
+        if (used + 1 < static_cast<size_t>(len)) std::snprintf(buf + used, len - used, "; per-env flexibility parameters");
+    }
     for (int j = 0; j < b->kp.n_proc; ++j) {
         const size_t used = std::strlen(buf);
         if (used + 1 >= static_cast<size_t>(len)) break;
@@ -693,6 +707,8 @@ int jb_set_model_variants(JbBatch* b, int32_t n_variants, const JbModelDesc* mod
     CU(cudaMemcpyAsync(d_vob, vob.data(), vob.size() * sizeof(int32_t), cudaMemcpyHostToDevice, b->stream));
     CU(cudaMemcpyAsync(d_bm, bm.data(), bm.size() * sizeof(double), cudaMemcpyHostToDevice, b->stream));
     CU(cudaStreamSynchronize(b->stream));   // the host vectors go away
+    b->h_variant_rows = rows;
+    b->h_variant_of_group = vob;
     b->kp.rdbl = d_rows; b->kp.n_variants = n_variants > 1 ? n_variants : 2;   // (a single variant still replaces the table: keep the indirection on)
     b->kp.rdbl_rows = static_cast<int32_t>(P0.rdbl.size());
     b->kp.variant_of_block = d_vob; b->kp.block_mass = d_bm;
@@ -700,6 +716,129 @@ int jb_set_model_variants(JbBatch* b, int32_t n_variants, const JbModelDesc* mod
 }
 
 int jb_envs_per_group(JbBatch* b) { return b ? 32 / b->plan.L : 0; }
+
+// Per-env flexibility parameters (the walker env's `model` randomisation, gym_jiminy locomotion.py:288-296): one row of
+// stiffness xyz | damping xyz per flexibility and env, read by the spherical records in place of RecDbl::motor[0..5].
+int jb_enable_per_env_flexibility(JbBatch* b, int32_t n_flex, const int32_t* flex_joints) {
+    if (!b) return fail(JB_ERR_INVALID_ARGUMENT, "null argument");
+    if (b->kp.flex_on) return fail(JB_ERR_INVALID_ARGUMENT, "per-env flexibility parameters are already enabled");
+    const Plan& P = b->plan;
+    const int L = P.L;
+    // the spherical joints of the plan, and the first (record, sub-lane) that holds each
+    std::vector<int> sph, sph_row;
+    for (int r = 0; r < P.nrec; ++r)
+        for (int s = 0; s < L; ++s) {
+            const RecInt& ri = P.rint[static_cast<size_t>(r) * L + s];
+            if (ri.kind == REC_SPH && std::find(sph.begin(), sph.end(), ri.joint) == sph.end()) {
+                sph.push_back(ri.joint);
+                sph_row.push_back(r * L + s);
+            }
+        }
+    if (sph.empty()) return fail(JB_ERR_INVALID_ARGUMENT, "the model has no flexibility joint");
+    std::vector<int> order;
+    if (flex_joints) {
+        if (n_flex != static_cast<int>(sph.size()))
+            return fail(JB_ERR_INVALID_ARGUMENT, "flex_joints must list every flexibility joint of the model once (" + std::to_string(sph.size()) + ")");
+        order.assign(flex_joints, flex_joints + n_flex);
+        for (int k = 0; k < n_flex; ++k)
+            if (std::find(sph.begin(), sph.end(), order[k]) == sph.end() || std::count(order.begin(), order.end(), order[k]) != 1)
+                return fail(JB_ERR_INVALID_ARGUMENT, "flex_joints must list every flexibility joint of the model once (joint " + std::to_string(order[k]) + ")");
+    } else {
+        order = sph;
+        std::sort(order.begin(), order.end());
+    }
+    const int nf = static_cast<int>(order.size());
+    std::vector<int32_t> of_rec(static_cast<size_t>(P.nrec) * L, -1);
+    for (int r = 0; r < P.nrec; ++r)
+        for (int s = 0; s < L; ++s) {
+            const RecInt& ri = P.rint[static_cast<size_t>(r) * L + s];
+            if (ri.kind == REC_SPH) of_rec[static_cast<size_t>(r) * L + s] = static_cast<int32_t>(std::find(order.begin(), order.end(), ri.joint) - order.begin());
+        }
+    // initial rows: each env's model values (the variant of its group, if any)
+    const int epw = 32 / L;
+    const bool variants = !b->h_variant_rows.empty();
+    std::vector<double> rows(static_cast<size_t>(b->n_env) * nf * 6);
+    for (int e = 0; e < b->n_env; ++e)
+        for (int k = 0; k < nf; ++k) {
+            const int row = sph_row[std::find(sph.begin(), sph.end(), order[k]) - sph.begin()];
+            const RecDbl& rd = variants ? b->h_variant_rows[static_cast<size_t>(b->h_variant_of_group[e / epw]) * P.rdbl.size() + row] : P.rdbl[row];
+            for (int i = 0; i < 6; ++i) rows[(static_cast<size_t>(e) * nf + k) * 6 + i] = rd.motor[i];
+        }
+    CU(cudaSetDevice(b->device));
+    int rc;
+    if ((rc = dev_alloc(b, &b->d_flex_pending, rows.size())) || (rc = dev_alloc(b, &b->d_flex_active, rows.size())) ||
+        (rc = dev_alloc(b, &b->d_flex_stage, rows.size())) || (rc = dev_alloc(b, &b->d_flex_bad, b->n_env)) ||
+        (rc = dev_alloc(b, &b->d_flex_of_rec, of_rec.size())))
+        return rc;
+    CU(cudaMemcpyAsync(b->d_flex_pending, rows.data(), rows.size() * sizeof(double), cudaMemcpyHostToDevice, b->stream));
+    CU(cudaMemcpyAsync(b->d_flex_active, rows.data(), rows.size() * sizeof(double), cudaMemcpyHostToDevice, b->stream));
+    CU(cudaMemcpyAsync(b->d_flex_of_rec, of_rec.data(), of_rec.size() * sizeof(int32_t), cudaMemcpyHostToDevice, b->stream));
+    CU(cudaStreamSynchronize(b->stream));   // the host vectors go away
+    KParams& kp = b->kp;
+    kp.flex_on = 1; kp.n_flex = nf;
+    kp.flex_of_rec = b->d_flex_of_rec; kp.flex_pending = b->d_flex_pending; kp.flex_active = b->d_flex_active; kp.flex_bad = b->d_flex_bad;
+    return JB_OK;
+}
+
+// Masked pending rows, one thread per env.  A row with a value that is not finite or is negative is not written and
+// flags its env (its next start refuses it); a valid row clears the flag.
+__global__ void set_flex_rows_kernel(double* __restrict__ pending, int32_t* __restrict__ bad_flag, const uint8_t* __restrict__ mask,
+                                     const double* __restrict__ rows, int n_env, int w) {
+    const int e = blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= n_env || (mask && !mask[e])) return;
+    const double* x = rows + static_cast<size_t>(e) * w;
+    bool bad = false;
+    for (int k = 0; k < w; ++k) bad = bad || !(x[k] >= 0.0 && x[k] <= 1.7976931348623157e308);
+    bad_flag[e] = bad ? 1 : 0;
+    if (bad) return;
+    double* row = pending + static_cast<size_t>(e) * w;
+    for (int k = 0; k < w; ++k) row[k] = x[k];
+}
+
+static int launch_flex_rows(JbBatch* b, const uint8_t* mask_dev, const double* rows) {
+    JB_LAUNCH(set_flex_rows_kernel, static_cast<unsigned>((b->n_env + 127) / 128), 128, 0, b->stream, b->d_flex_pending,
+              b->d_flex_bad, mask_dev, rows, b->n_env, 6 * b->kp.n_flex);
+    CU(cudaGetLastError());
+    ++b->launches;
+    return JB_OK;
+}
+
+int jb_set_flexibility_env(JbBatch* b, const uint8_t* mask, const double* rows) {
+    if (!b || !rows) return fail(JB_ERR_INVALID_ARGUMENT, "null argument");
+    if (!b->kp.flex_on) return fail(JB_ERR_BAD_CONTROL_FLOW, "per-env flexibility parameters are not enabled (jb_enable_per_env_flexibility)");
+    CU(cudaSetDevice(b->device));
+    const int w = 6 * b->kp.n_flex;
+    for (int e = 0; e < b->n_env; ++e) {
+        if (mask && !mask[e]) continue;
+        for (int k = 0; k < w; ++k) {
+            const double x = rows[static_cast<size_t>(e) * w + k];
+            if (!std::isfinite(x)) return fail(JB_ERR_INVALID_ARGUMENT, "flexibility stiffness / damping must be finite (env " + std::to_string(e) + ").");
+            if (x < 0.0) return fail(JB_ERR_INVALID_ARGUMENT, "All stiffness and damping coefficients of flexibility joints must be positive (env " + std::to_string(e) + ").");
+        }
+    }
+    CU(cudaMemcpyAsync(b->d_flex_stage, rows, static_cast<size_t>(b->n_env) * w * sizeof(double), cudaMemcpyHostToDevice, b->stream));
+    if (mask) CU(cudaMemcpyAsync(b->d_mask, mask, b->n_env, cudaMemcpyHostToDevice, b->stream));
+    int rc = launch_flex_rows(b, mask ? b->d_mask : nullptr, b->d_flex_stage);
+    if (rc) return rc;
+    CU(cudaStreamSynchronize(b->stream));
+    return JB_OK;
+}
+
+int jb_set_flexibility_env_device(JbBatch* b, const uint8_t* mask_dev, const double* rows_dev) {
+    if (!b || !rows_dev) return fail(JB_ERR_INVALID_ARGUMENT, "null argument");
+    if (!b->kp.flex_on) return fail(JB_ERR_BAD_CONTROL_FLOW, "per-env flexibility parameters are not enabled (jb_enable_per_env_flexibility)");
+    CU(cudaSetDevice(b->device));
+    return launch_flex_rows(b, mask_dev, rows_dev);
+}
+
+int jb_get_flexibility_env(JbBatch* b, double* out) {
+    if (!b || !out) return fail(JB_ERR_INVALID_ARGUMENT, "null argument");
+    if (!b->kp.flex_on) return fail(JB_ERR_BAD_CONTROL_FLOW, "per-env flexibility parameters are not enabled (jb_enable_per_env_flexibility)");
+    CU(cudaSetDevice(b->device));
+    CU(cudaMemcpyAsync(out, b->d_flex_active, static_cast<size_t>(b->n_env) * 6 * b->kp.n_flex * sizeof(double), cudaMemcpyDeviceToHost, b->stream));
+    CU(cudaStreamSynchronize(b->stream));
+    return JB_OK;
+}
 
 // Linear internal dynamics u_custom = -k q - d v on 1-dof joints: the device-side stand-in for the
 // `internalDynamics` functor of FunctionalController (controller_functor.h:27-80).

@@ -186,6 +186,13 @@ struct KParams {
     const double* sp_env_pending;  // [n_env][stride] rows written by the setters
     double* sp_env_opt;            // [n_env][stride] rows latched at the env's last start
     int32_t* sp_env_bad;           // [n_env] 1: the last device row was rejected, the env's next start refuses it
+    // per-env flexibility parameters (jb_enable_per_env_flexibility): stiffness xyz | damping xyz of every flexibility,
+    // one row [n_flex][6] per env, read by the spherical records in place of RecDbl::motor[0..5]
+    int32_t flex_on, n_flex;
+    const int32_t* flex_of_rec;    // [nrec][L] flexibility index of the spherical record on that sub-lane, -1 elsewhere
+    const double* flex_pending;    // [n_env][n_flex][6] rows written by the setters
+    double* flex_active;           // [n_env][n_flex][6] rows latched at the env's last start
+    int32_t* flex_bad;             // [n_env] 1: the last device row was rejected, the env's next start refuses it
 };
 
 // Launch parameters live in constant memory (uniform constant-bank operands in every device
@@ -832,6 +839,23 @@ struct SigQuadrupedT {
 using SigQuadruped = SigQuadrupedT<false>;
 using SigQuadrupedCons = SigQuadrupedT<true>;
 
+// Per-env flexibility parameters (jb_enable_per_env_flexibility) are read by sweep instances of their own,
+// SigDynamicFlex, which only the full body of env_step_kernel_flex calls (the kernel of every launch of such a batch):
+// the kernels and sweeps every other batch runs stay as they were.
+template <bool UNIFORM, bool EXT>
+struct SigDynamicFlex : SigDynamic<UNIFORM, EXT> {};
+template <class SIG> struct sig_has_flex { static constexpr bool value = false; };
+template <bool UNIFORM, bool EXT> struct sig_has_flex<SigDynamicFlex<UNIFORM, EXT>> { static constexpr bool value = true; };
+// Stiffness xyz | damping xyz of the spherical record r on this lane: the record's table row (the batch's model or the
+// block's variant), or, in the SigDynamicFlex instances, the env's active row
+template <class SIG>
+JB_DI const double* flex_params(const Ctx& c, int r, int L, const RecDbl* rd) {
+    if constexpr (sig_has_flex<SIG>::value)
+        return KP->flex_active + (static_cast<size_t>(c.env) * KP->n_flex + KP->flex_of_rec[r * L + c.sub]) * 6;
+    else
+        return rd->motor;
+}
+
 template <class SIG>
 JB_DI bool rhs_impl(const Ctx c, const bool up_to_date, int* status) {
     const int L = SIG::lanes();
@@ -990,12 +1014,13 @@ JB_DI bool rhs_impl(const Ctx c, const bool up_to_date, int* status) {
                 const double qs[4] = {RP(RF_QS + 3), RP(RF_QS + 4), RP(RF_QS + 5), RP(RF_QS + 6)};
                 double angle;
                 const V3 aa = quat_log3(qs, angle);
-                const V3 t = jlog3_mul(angle, aa, mk(rd->motor[0] * aa.x, rd->motor[1] * aa.y, rd->motor[2] * aa.z));
+                const double* fx = flex_params<SIG>(c, r, L, rd);
+                const V3 t = jlog3_mul(angle, aa, mk(fx[0] * aa.x, fx[1] * aa.y, fx[2] * aa.z));
                 const bool zero = SIG::has_cons && (c.flags & CTX_ZERO_U);
                 double* const xp = rp + KP->sph_off * 32;
-                xp[(RS_TAU + 0) * 32] = zero ? 0.0 : (0.0 - t.x) - rd->motor[3] * vJ.a.x;
-                xp[(RS_TAU + 1) * 32] = zero ? 0.0 : (0.0 - t.y) - rd->motor[4] * vJ.a.y;
-                xp[(RS_TAU + 2) * 32] = zero ? 0.0 : (0.0 - t.z) - rd->motor[5] * vJ.a.z;
+                xp[(RS_TAU + 0) * 32] = zero ? 0.0 : (0.0 - t.x) - fx[3] * vJ.a.x;
+                xp[(RS_TAU + 1) * 32] = zero ? 0.0 : (0.0 - t.y) - fx[4] * vJ.a.y;
+                xp[(RS_TAU + 2) * 32] = zero ? 0.0 : (0.0 - t.z) - fx[5] * vJ.a.z;
                 sm_store_xf(c, base + RF_LIMI, li);
                 sm_store_mot(c, base + RF_F, f);
                 sm_store_mot(c, base + KP->sph_off + RS_BIAS, bias);
@@ -1314,6 +1339,11 @@ __device__ __noinline__ bool rhs_static_quadruped(const Ctx c, const bool up_to_
 // the same sweeps with the `constraint` contact model (contact frames handed to the constraint solver, start-time flags)
 __device__ __noinline__ bool rhs_static_quadruped_cons(const Ctx c, const bool up_to_date, int* status) {
     return rhs_impl<SigQuadrupedCons>(c, up_to_date, status);
+}
+template <bool EXT>
+__device__ __noinline__ bool rhs_dynamic_flex(const Ctx c, const bool up_to_date, int* status) {
+    if (KP->all_uniform) return rhs_impl<SigDynamicFlex<true, EXT>>(c, up_to_date, status);
+    return rhs_impl<SigDynamicFlex<false, EXT>>(c, up_to_date, status);
 }
 template <bool EXT>
 __device__ __noinline__ bool rhs_dynamic(const Ctx c, const bool up_to_date, int* status) {
@@ -1969,11 +1999,18 @@ __device__ __noinline__ void eval_process_forces(const Ctx c, double t) {
 // The same at a stage of a step, `t + w` (w = c_i dt of the tableau).  Only the steppers of SigDynamicProc, the signature
 // of batches with process forces, carry it: the instances every other batch runs stay as they were.
 struct SigDynamicProc : SigDynamic<false> {};
+// the steppers of batches with per-env flexibility parameters (env_step_kernel_flex): the full body's sweeps with the
+// env's active rows, and process forces at every stage time when the batch has any
+struct SigDynamicFlexStep : SigDynamic<false> {};
 template <class SIG> struct sig_has_proc { static constexpr bool value = false; };
 template <> struct sig_has_proc<SigDynamicProc> { static constexpr bool value = true; };
+template <class SIG> struct sig_flex_step { static constexpr bool value = false; };
+template <> struct sig_flex_step<SigDynamicFlexStep> { static constexpr bool value = true; };
 template <class SIG>
 JB_DI void eval_process_stage(const Ctx& c, double w) {
     if constexpr (sig_has_proc<SIG>::value) eval_process_forces(c, SMF(c, proc_time_field()) + w);
+    // (the time field exists only behind the slots of a registered process force)
+    else if constexpr (sig_flex_step<SIG>::value) { if (KP->n_proc > 0) eval_process_forces(c, SMF(c, proc_time_field()) + w); }
 }
 // The force-carrying hot path of the quadruped signature (env_step_kernel_ext): the plan of SigQuadruped, evaluated by
 // quadruped_crba<., true>, with the process forces of update period 0 at every stage time.  A type of its own, so that
@@ -1988,6 +2025,7 @@ template <> struct sig_is_fast_ext<FastOf<SigQuadrupedExt>> { static constexpr b
 // (Engine::computeAcceleration with enabled constraints, engine.cc:3709-3866) corrects them if needed.
 // Joint position bounds (computePositionLimitsForcesAlgo, engine.cc:3253-3338): leaving [lo, hi] enables the
 // joint's constraint; the update also runs while this lane owns enabled constraints (they may switch off).
+template <bool FLEX = false>
 JB_DI void rhs(const Ctx c, const bool up_to_date, int* status) {
     JB_PROF_T(t_rhs);
     JB_PROF_COUNT(8, 1);                                   // calls of rhs() per warp (each diverged subset counts)
@@ -1996,7 +2034,7 @@ JB_DI void rhs(const Ctx c, const bool up_to_date, int* status) {
     const bool out = (KP->sig_id == SigQuadruped::ID)
                          ? (KP->opt.contact_model == JB_CONTACT_CONSTRAINT ? rhs_static_quadruped_cons(c, up_to_date, status)
                                                                            : rhs_static_quadruped(c, up_to_date, status))
-                         : rhs_dynamic<true>(c, up_to_date, status);
+                         : (FLEX ? rhs_dynamic_flex<true>(c, up_to_date, status) : rhs_dynamic<true>(c, up_to_date, status));
     JB_PROF_ADD(0, t_rhs);                                 // the sweeps
     if (!KP->cons_on) { if (out) *status |= JB_ENV_JOINT_LIMIT; return; }
     JB_PROF_T(t_upd);
@@ -2046,7 +2084,7 @@ template <class SIG>
 JB_DI void rhs_sig(const Ctx c, const bool up_to_date, int* status) {
     if constexpr (sig_is_fast_ext<SIG>::value) rhs_fast_ext(c, up_to_date, status);
     else if constexpr (sig_is_fast<SIG>::value) rhs_fast(c, up_to_date, status);
-    else rhs(c, up_to_date, status);
+    else rhs<sig_flex_step<SIG>::value>(c, up_to_date, status);
 }
 // one-call RK4 stage of the quadruped hot path, with or without the force slots
 template <class SIG>
@@ -2337,9 +2375,11 @@ JB_DI bool accel_has_nan(const Ctx& c) {
     return accel_has_nan_t<SigDynamic<false>>(c);
 }
 // EXT (with FAST): the force-carrying hot path, quadruped signature only
-template <bool FAST, bool EXT = false>
+template <bool FAST, bool EXT = false, bool FLEX = false>
 JB_DI void step_euler(const Ctx c, double dt, int* status) {
-    if constexpr (EXT) {
+    if constexpr (FLEX) {
+        step_euler_t<SigDynamicFlexStep>(c, dt, status);
+    } else if constexpr (EXT) {
         step_euler_t<FastOf<SigQuadrupedExt>>(c, dt, status);
     } else if constexpr (FAST) {
         if (KP->sig_id == SigQuadruped::ID) step_euler_t<FastOf<SigQuadruped>>(c, dt, status);
@@ -2350,9 +2390,11 @@ JB_DI void step_euler(const Ctx c, double dt, int* status) {
         else step_euler_t<SigDynamic<false>>(c, dt, status);
     }
 }
-template <bool FAST, bool EXT = false>
+template <bool FAST, bool EXT = false, bool FLEX = false>
 JB_DI void step_rk4(const Ctx c, double dt, int* status) {
-    if constexpr (EXT) {
+    if constexpr (FLEX) {
+        step_rk4_t<SigDynamicFlexStep>(c, dt, status);
+    } else if constexpr (EXT) {
         step_rk4_t<FastOf<SigQuadrupedExt>>(c, dt, status);
     } else if constexpr (FAST) {
         if (KP->sig_id == SigQuadruped::ID) step_rk4_t<FastOf<SigQuadruped>>(c, dt, status);
@@ -2451,6 +2493,7 @@ JB_DI double difference_so2(double c0, double s0, double c1, double s1) {
 }
 
 // returns 0 = success, 1 = failure (step rejected, dt shrunk), 2 = error (NaN)
+template <bool FLEX = false>
 __device__ __noinline__ int step_dopri(const Ctx c, double* dt_io, int* status) {
     const int L = KP->L;
     const double h = *dt_io;
@@ -2493,7 +2536,7 @@ __device__ __noinline__ int step_dopri(const Ctx c, double* dt_io, int* status) 
             }
         }
         if (KP->n_proc > 0) eval_process_forces(c, SMF(c, proc_time_field()) + dopri::Cn[i] * h);
-        rhs(c, false, status);
+        rhs<FLEX>(c, false, status);
         for (int r = 0; r < KP->nrec; ++r) {
             const RecInt* ri = KP->rint + (r * L + c.sub);
             if (ri->kind == REC_PAD) continue;

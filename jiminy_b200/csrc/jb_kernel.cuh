@@ -238,10 +238,11 @@ __device__ __noinline__ void store_outputs(const Ctx c) {
                 const double qa[4] = {RP(RF_Q + 3), RP(RF_Q + 4), RP(RF_Q + 5), RP(RF_Q + 6)};
                 double angle;
                 const V3 aa = quat_log3(qa, angle);
-                const V3 t = jlog3_mul(angle, aa, mk(rd->motor[0] * aa.x, rd->motor[1] * aa.y, rd->motor[2] * aa.z));
-                KP->eff_u[col * KP->nv + ri->idx_v + 0] = (0.0 - t.x) - rd->motor[3] * RP(RF_V + 3);
-                KP->eff_u[col * KP->nv + ri->idx_v + 1] = (0.0 - t.y) - rd->motor[4] * RP(RF_V + 4);
-                KP->eff_u[col * KP->nv + ri->idx_v + 2] = (0.0 - t.z) - rd->motor[5] * RP(RF_V + 5);
+                const double* fx = KP->flex_on ? flex_params<SigDynamicFlex<false, true>>(c, r, L, rd) : rd->motor;
+                const V3 t = jlog3_mul(angle, aa, mk(fx[0] * aa.x, fx[1] * aa.y, fx[2] * aa.z));
+                KP->eff_u[col * KP->nv + ri->idx_v + 0] = (0.0 - t.x) - fx[3] * RP(RF_V + 3);
+                KP->eff_u[col * KP->nv + ri->idx_v + 1] = (0.0 - t.y) - fx[4] * RP(RF_V + 4);
+                KP->eff_u[col * KP->nv + ri->idx_v + 2] = (0.0 - t.z) - fx[5] * RP(RF_V + 5);
             }
         } else if (ri->kind == REC_FREE) {
 #pragma unroll
@@ -313,10 +314,11 @@ __device__ __noinline__ void store_dynamics(const Ctx c) {
                 const double qa[4] = {RP(RF_QS + 3), RP(RF_QS + 4), RP(RF_QS + 5), RP(RF_QS + 6)};
                 double angle;
                 const V3 aa = quat_log3(qa, angle);
-                const V3 t = jlog3_mul(angle, aa, mk(rd->motor[0] * aa.x, rd->motor[1] * aa.y, rd->motor[2] * aa.z));
-                KP->u_out[col * KP->nv + ri->idx_v + 0] = (0.0 - t.x) - rd->motor[3] * RP(RF_VS + 3);
-                KP->u_out[col * KP->nv + ri->idx_v + 1] = (0.0 - t.y) - rd->motor[4] * RP(RF_VS + 4);
-                KP->u_out[col * KP->nv + ri->idx_v + 2] = (0.0 - t.z) - rd->motor[5] * RP(RF_VS + 5);
+                const double* fx = KP->flex_on ? flex_params<SigDynamicFlex<false, true>>(c, r, L, rd) : rd->motor;
+                const V3 t = jlog3_mul(angle, aa, mk(fx[0] * aa.x, fx[1] * aa.y, fx[2] * aa.z));
+                KP->u_out[col * KP->nv + ri->idx_v + 0] = (0.0 - t.x) - fx[3] * RP(RF_VS + 3);
+                KP->u_out[col * KP->nv + ri->idx_v + 1] = (0.0 - t.y) - fx[4] * RP(RF_VS + 4);
+                KP->u_out[col * KP->nv + ri->idx_v + 2] = (0.0 - t.z) - fx[5] * RP(RF_VS + 5);
             }
         } else if (ri->kind == REC_FREE) {
 #pragma unroll
@@ -367,7 +369,9 @@ __device__ __noinline__ void store_dynamics(const Ctx c) {
 // EXT = true (with FAST): the force-carrying hot path of the quadruped signature (env_step_kernel_ext).  Everything the
 // full body does for impulse / profile / process forces runs here too: slots zeroed at load, refreshed at every
 // scheduler iteration (impulse breakpoints, FSAL repair on a change), process forces before every evaluation.
-template <bool FAST, bool EXT = false>
+// FLEX (full body only): the batch has per-env flexibility parameters (env_step_kernel_flex): each start latches the
+// env's pending row, and the sweeps read the active rows.
+template <bool FAST, bool EXT = false, bool FLEX = false>
 __device__ __forceinline__ void env_step_body(const LaunchArgs& la, const bool only_flagged) {
     static_assert(FAST || !EXT, "external forces on the full body need no instance of their own");
     Ctx c;
@@ -409,6 +413,19 @@ __device__ __forceinline__ void env_step_body(const LaunchArgs& la, const bool o
         if (mode == MODE_START && KP->sp_env_on && KP->sp_env_bad[c.env] != 0) {
             if (c.valid && c.sub == 0) KP->status[c.env] = JB_ENV_NOT_STARTED | JB_ENV_BAD_START;
             return;
+        }
+        // per-env flexibility parameters: refused if the last device row for this env was, else the pending row becomes
+        // the one the episode runs with (setOptions before Engine::reset), before the start's own evaluations
+        if (FLEX && mode == MODE_START) {
+            if (KP->flex_bad[c.env] != 0) {
+                if (c.valid && c.sub == 0) KP->status[c.env] = JB_ENV_NOT_STARTED | JB_ENV_BAD_START;
+                return;
+            }
+            if (c.valid) {
+                const size_t o = static_cast<size_t>(c.env) * KP->n_flex * 6;
+                for (int k = c.sub; k < 6 * KP->n_flex; k += L) KP->flex_active[o + k] = KP->flex_pending[o + k];
+            }
+            jb_syncwarp(c);
         }
     }
     if (mode == MODE_STEP && (status & (JB_ENV_NOT_STARTED | JB_ENV_NAN | JB_ENV_ITER_FAILED | JB_ENV_DT_UNDERFLOW | JB_ENV_SOLVER_FAILED))) {
@@ -472,7 +489,7 @@ __device__ __forceinline__ void env_step_body(const LaunchArgs& la, const bool o
     if (!FAST && mode == MODE_DYNAMICS) {
         stage_from_accepted(c);
         int st = 0;
-        rhs(c, false, &st);
+        rhs<FLEX>(c, false, &st);
         store_dynamics(c);
         return;
     }
@@ -497,11 +514,11 @@ __device__ __forceinline__ void env_step_body(const LaunchArgs& la, const bool o
             // solver warm-started on an up-to-date state
             cons_reset(c);
             Ctx c0 = c; c0.flags |= CTX_ZERO_U | CTX_IGNORE_BOUNDS;
-            rhs(c0, false, &status);
+            rhs<FLEX>(c0, false, &status);
             const bool constrained = jb_any(c, SMF(c, KP->cons_off) != 0.0);
             Ctx c1 = c; c1.flags |= CTX_START_FEEDBACK;
-            for (int it = 1; it < (constrained ? 4 : 2); ++it) rhs(c1, true, &status);
-        } else rhs(c, false, &status);
+            for (int it = 1; it < (constrained ? 4 : 2); ++it) rhs<FLEX>(c1, true, &status);
+        } else rhs<FLEX>(c, false, &status);
         // forceMax > 1e5 guard (engine.cc:1310-1346)
         double fmax2 = 0.0;
         for (int k = 0; k < KP->ncslot; ++k) {
@@ -558,9 +575,9 @@ __device__ __forceinline__ void env_step_body(const LaunchArgs& la, const bool o
             if constexpr (!FAST || EXT) {
                 if (KP->n_proc > 0) SMF(c, proc_time_field()) = t;   // stage times of the process forces
             }
-            if (opt.ode_solver == JB_SOLVER_EULER_EXPLICIT) { step_euler<FAST, EXT>(c, dtLargest, &status); dtLargest = D_INF; }
-            else if (FAST || opt.ode_solver == JB_SOLVER_RUNGE_KUTTA_4) { step_rk4<FAST, EXT>(c, dtLargest, &status); dtLargest = D_INF; }
-            else { if constexpr (!FAST) rc = step_dopri(c, &dtLargest, &status); }
+            if (opt.ode_solver == JB_SOLVER_EULER_EXPLICIT) { step_euler<FAST, EXT, FLEX>(c, dtLargest, &status); dtLargest = D_INF; }
+            else if (FAST || opt.ode_solver == JB_SOLVER_RUNGE_KUTTA_4) { step_rk4<FAST, EXT, FLEX>(c, dtLargest, &status); dtLargest = D_INF; }
+            else { if constexpr (!FAST) rc = step_dopri<FLEX>(c, &dtLargest, &status); }
             need_refresh = false;
             if constexpr (FAST) {
                 // one vote for the two rare events of a step: NaN in the new acceleration, or a joint that left its
@@ -616,7 +633,7 @@ __device__ __forceinline__ void env_step_body(const LaunchArgs& la, const bool o
                 stage_from_accepted<EXT>(c);
                 if constexpr (!FAST || EXT) { if (KP->n_proc > 0) eval_process_forces(c, t); }
                 if constexpr (EXT) rhs_fast_ext(c, !need_refresh, &status);
-                else if constexpr (FAST) rhs_fast(c, !need_refresh, &status); else rhs(c, !need_refresh, &status);
+                else if constexpr (FAST) rhs_fast(c, !need_refresh, &status); else rhs<FLEX>(c, !need_refresh, &status);
                 need_refresh = false;
                 hasDynamicsChanged = false;
             }
@@ -633,7 +650,7 @@ __device__ __forceinline__ void env_step_body(const LaunchArgs& la, const bool o
                         stage_from_accepted<EXT>(c);
                         if constexpr (!FAST || EXT) { if (KP->n_proc > 0) eval_process_forces(c, t); }
                         if constexpr (EXT) rhs_fast_ext(c, !need_refresh, &status);
-                        else if constexpr (FAST) rhs_fast(c, !need_refresh, &status); else rhs(c, !need_refresh, &status);
+                        else if constexpr (FAST) rhs_fast(c, !need_refresh, &status); else rhs<FLEX>(c, !need_refresh, &status);
                         need_refresh = false;
                         hasDynamicsChanged = false;
                     }
@@ -765,19 +782,20 @@ JB_DI unsigned int jb_smid() {
 
 // The full body: every mode, every stepper, the constraint path.  Out of line, so that the hot-path kernel carries one
 // call to it instead of a second copy of the code.
+template <bool FLEX = false>
 __device__ __noinline__ void env_step_full(const LaunchArgs la, const bool only_flagged) {
     // constraint workspace of this block: one row per block of the launch.  (A pool of per-SM slots taken with an atomic
     // spin by lane 0 kept the workspace L2-resident, but left the warp's env groups running one after the other in the
     // constraint solvers -- several times slower on ANYmal with constraint contacts.)
     if (threadIdx.x == 0) jb_cw_slot = static_cast<int>(blockIdx.x);
     __syncwarp();
-    env_step_body<false>(la, only_flagged);
+    env_step_body<false, false, FLEX>(la, only_flagged);
 }
 
 // One launch = one Engine::step (or start / single evaluation) of every env.  FAST: the hot-path body first; the envs it
 // handed over (a joint left its bounds now, or constraints still enabled from an earlier step) go through the full
 // body in the same launch, so a step is always exactly one kernel.  EXT: the hot-path body is the force-carrying one.
-template <bool FAST, bool EXT>
+template <bool FAST, bool EXT, bool FLEX = false>
 __device__ __forceinline__ void env_step_launch(const LaunchArgs& la) {
     JB_PROF_T(t_kernel);
     if constexpr (FAST) {
@@ -785,7 +803,7 @@ __device__ __forceinline__ void env_step_launch(const LaunchArgs& la) {
         __syncwarp();   // needs_full is written by sub-lane 0 of each env
         const int flag = KP->needs_full[blockIdx.x * (32 / KP->L) + (threadIdx.x & 31) / KP->L];
         if (__any_sync(0xffffffffu, flag != 0)) env_step_full(la, true);
-    } else env_step_full(la, false);
+    } else env_step_full<FLEX>(la, false);
     JB_PROF_ADD(6, t_kernel);                              // the whole kernel
     JB_PROF_COUNT(7, 1);                                   // warps
 #ifndef JB_HOST_EMUL
@@ -810,6 +828,9 @@ __global__ void __launch_bounds__(32) env_step_kernel_t(const LaunchArgs la) { e
 // Batches of the quadruped signature with external forces (composite-rigid-body evaluation, spring-damper contacts,
 // Euler / RK4): the forces ride the hot path, the envs it hands over run the full body's force-aware generic sweeps.
 __global__ void __launch_bounds__(32) env_step_kernel_ext(const LaunchArgs la) { env_step_launch<true, true>(la); }
+// Batches with per-env flexibility parameters (jb_enable_per_env_flexibility): every launch runs the full body with the
+// sweep instances that read the env's active rows (SigDynamicFlex), so the kernels above are not touched.
+__global__ void __launch_bounds__(32) env_step_kernel_flex(const LaunchArgs la) { env_step_launch<false, false, true>(la); }
 
 // ---- observation exchange over peer memory: the consumer's wait (one thread)
 #ifndef JB_HOST_EMUL

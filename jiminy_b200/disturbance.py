@@ -181,13 +181,13 @@ class WalkerDisturbance:
 
 def from_std_ratio(robot, std_ratio: Optional[dict], simulation_duration_max: float) -> Optional[WalkerDisturbance]:
     """The disturbance an env's `std_ratio` asks for: None or {} -> none, {"disturbance": r} -> the walker disturbance
-    (none when r == 0 or absent).  "sensors" is `sensor_randomisation.from_std_ratio`'s; the other keys of the reference
-    (ground, model, flexibility) are not implemented."""
+    (none when r == 0 or absent).  "sensors" is `sensor_randomisation.from_std_ratio`'s and "model"
+    `model_randomisation.from_std_ratio`'s; the other keys of the reference (ground, flexibility) are not implemented."""
     if not std_ratio:
         return None
-    other = sorted(set(std_ratio) - {"disturbance", "sensors"})
+    other = sorted(set(std_ratio) - {"disturbance", "sensors", "model"})
     if other:
-        raise NotImplementedError(f"std_ratio keys not supported by the batched envs: {other} (only 'disturbance' and 'sensors')")
+        raise NotImplementedError(f"std_ratio keys not supported by the batched envs: {other} (only 'disturbance', 'sensors' and 'model')")
     r = float(std_ratio.get("disturbance", 0.0))
     if r < 0.0:
         raise ValueError("std_ratio['disturbance'] must be positive")

@@ -21,7 +21,7 @@ from typing import Any, Dict, Optional, Tuple
 
 import numpy as np
 
-from . import core, scenarios, sensor_randomisation
+from . import core, model_randomisation, scenarios, sensor_randomisation
 from .disturbance import from_std_ratio
 from .model import RobotTable
 
@@ -105,7 +105,9 @@ class BatchedJiminyEnv:
                  simulation_duration_max: float = 20.0, api_: Optional[core.Api] = None, std_ratio: Optional[dict] = None):
         """`std_ratio`: the reference walker env's randomisation ratios.  None or {}: none; "disturbance": r, the walker
         disturbance forces (`jiminy_b200.disturbance`); "sensors": r, noise, bias, delay and jitter of every sensor and a
-        new seed of its generators (`jiminy_b200.sensor_randomisation`).  Both are re-drawn for every env that (re)starts."""
+        new seed of its generators (`jiminy_b200.sensor_randomisation`); "model": r, stiffness and damping of every
+        flexibility joint (`jiminy_b200.model_randomisation`; NotImplementedError on a robot without one).  All are re-drawn for every
+        env that (re)starts."""
         self.sc = scenario
         self.robot: RobotTable = scenario.robot
         self.n_env, self.step_dt = scenario.n_env, scenario.step_dt
@@ -134,6 +136,11 @@ class BatchedJiminyEnv:
             self.sensor_randomisation.register(self.engine)
             self._sensor_rng = np.random.default_rng([scenario.seed, 0x5E45])
             self.sensor_rows: Optional[Dict[str, np.ndarray]] = None      # the options and seed every env runs with
+        self.model_randomisation = model_randomisation.from_std_ratio(self.robot, std_ratio)
+        if self.model_randomisation is not None:
+            self.model_randomisation.register(self.engine)
+            self._model_rng = np.random.default_rng([scenario.seed, 0xF1E8])
+            self.model_rows: Optional[np.ndarray] = None     # the flexibility rows every env runs with [n_env, n_flex, 6]
         self._started = False
 
     # ------------------------------------------------------------------ helpers
@@ -169,6 +176,15 @@ class BatchedJiminyEnv:
             self.sensor_rows = draw
             self.sensor_randomisation.apply_host(self.engine, draw, mask)
 
+    def _redraw_model(self, mask: Optional[np.ndarray]) -> None:
+        """New flexibility stiffness and damping for the envs about to (re)start (`_setup`, locomotion.py:288-296)."""
+        if self.model_randomisation is not None:
+            draw = self.model_randomisation.draw_numpy(self._model_rng, self.n_env)
+            if mask is not None and self.model_rows is not None:
+                draw = np.where(np.asarray(mask).astype(bool)[:, None, None], draw, self.model_rows)
+            self.model_rows = draw
+            self.model_randomisation.apply_host(self.engine, draw, mask)
+
     # ------------------------------------------------------------------ gym API
     def reset(self, mask: Optional[np.ndarray] = None) -> Tuple[Dict[str, Any], Dict[str, Any]]:
         if mask is None or not self._started:
@@ -176,6 +192,7 @@ class BatchedJiminyEnv:
             self.engine.set_command(self.sc.target0)
             self._redraw_disturbance(None)
             self._redraw_sensors(None)
+            self._redraw_model(None)
             self.engine.start(q0, v0)
             self.num_steps[:] = 0
             self._started = True
@@ -183,6 +200,7 @@ class BatchedJiminyEnv:
             q0, v0 = self._sample_state(self.n_env)
             self._redraw_disturbance(mask)
             self._redraw_sensors(mask)
+            self._redraw_model(mask)
             self.engine.start(q0, v0, mask=mask)
             self.num_steps[mask.astype(bool)] = 0
         return self._observation(), {}
@@ -251,6 +269,7 @@ class PDControlBatchedEnv(BatchedJiminyEnv):
             q0, v0 = (self.sc.q0, self.sc.v0) if not self._started else self._sample_state(self.n_env)
             self._redraw_disturbance(None)
             self._redraw_sensors(None)
+            self._redraw_model(None)
             self.engine.start(q0, v0)
             self.num_steps[:] = 0
             self._started = True

@@ -32,6 +32,11 @@ the done mask are re-drawn the same way (`jiminy_b200.sensor_randomisation`) and
 `env.sensor_rows` holds the options and seed every env currently runs with.  The sampler never draws a row the setter
 would reject (its delays stay below the bound the buffer was sized for).
 
+Model.  With `std_ratio={"model": r}` the stiffness and damping of every flexibility joint of the envs in the done mask are
+re-drawn the same way (`jiminy_b200.model_randomisation`) and written by `jb_set_flexibility_env_device` before the
+masked restart, which latches them.  `env.model_rows` holds the rows every env currently runs with.  The sampler never
+draws a row the setter would reject (the ratio is checked against the nominal values at construction).
+
 Streams.  All work runs on the batch's own stream (`torch.cuda.ExternalStream(engine.stream())`).  On entry it waits
 for the caller's current stream; on exit the caller's current stream waits for it.  With the CPU emulation of the
 library (`api_` given), device memory is host memory: the env then runs on `torch_device="cpu"`, without streams.
@@ -111,6 +116,11 @@ class DeviceBatchedEnv(envs.BatchedJiminyEnv):
             self._sensor_gen.manual_seed(int(np.random.default_rng([self.sc.seed, 0x5E45]).integers(0, 2 ** 31 - 1)))
             with self._on_batch_stream():
                 self.sensor_rows = self.sensor_randomisation.draw_torch(self._sensor_gen, n, dev)
+        if self.model_randomisation is not None:
+            self._model_gen = torch.Generator(device=dev)
+            self._model_gen.manual_seed(int(np.random.default_rng([self.sc.seed, 0xF1E8]).integers(0, 2 ** 31 - 1)))
+            with self._on_batch_stream():
+                self.model_rows = self.model_randomisation.draw_torch(self._model_gen, n, dev)
         self.num_steps = torch.zeros(n, dtype=torch.int64, device=dev)
         # zero-copy views of the batch's device buffers
         ptr = eng.device_state_ptrs()
@@ -209,6 +219,15 @@ class DeviceBatchedEnv(envs.BatchedJiminyEnv):
             rows[k].copy_(new[k] if done is None else torch.where(done.view(-1, *([1] * (rows[k].dim() - 1))), new[k], rows[k]))
         self.sensor_randomisation.apply_device(self.engine, rows, None if done is None else self._mask.data_ptr())
 
+    def _redraw_model(self, done: Optional[torch.Tensor]) -> None:
+        """New flexibility stiffness and damping for the envs of `done` (None: all), drawn on the device and written by the
+        device setter with the mask in `self._mask`; `model_rows` keeps what every env runs with."""
+        if self.model_randomisation is None:
+            return
+        new = self.model_randomisation.draw_torch(self._model_gen, self.n_env, self.torch_device)
+        self.model_rows.copy_(new if done is None else torch.where(done.view(-1, 1, 1), new, self.model_rows))
+        self.model_randomisation.apply_device(self.engine, self.model_rows, None if done is None else self._mask.data_ptr())
+
     def _restart(self, done: torch.Tensor) -> torch.Tensor:
         """Masked restart of the envs in `done` from bank rows drawn on the device; returns the rows (-1: not restarted)."""
         q_bank, v_bank = self.reset_states
@@ -218,6 +237,7 @@ class DeviceBatchedEnv(envs.BatchedJiminyEnv):
         self._mask.copy_(done)
         self._redraw_disturbance(done)
         self._redraw_sensors(done)
+        self._redraw_model(done)
         self.engine.start_device(self._q_start.data_ptr(), self._v_start.data_ptr(), self._mask.data_ptr())
         self.num_steps.masked_fill_(done, 0)
         return torch.where(done, rows, torch.full_like(rows, -1))
@@ -232,6 +252,7 @@ class DeviceBatchedEnv(envs.BatchedJiminyEnv):
                 self._first_command()
                 self._redraw_disturbance(None)
                 self._redraw_sensors(None)
+                self._redraw_model(None)
                 self.engine.start(self.sc.q0, self.sc.v0)
                 self.num_steps.zero_()
                 self._started = True

@@ -25,8 +25,13 @@ forces ride the quadruped hot path (`env_step_kernel_ext`); Atlas runs the gener
 and jitter of every sensor and fresh generator seeds, re-drawn at every restart); with both options both are on in the
 "on" runs.
 
-    python tools/bench_pipeline.py [--robot atlas|anymal] [--loop host|device] [--alternate R] [--n-env 4096]
-                                   [--steps 10] [--warmup 3] [--duration-max 0.4] [--disturbance R] [--sensors R]
+`--robot anymal_flexible` is the ANYmal configuration on the robot with a flexibility joint in every leg, and `--model R`
+turns the walker model randomisation on the same way (`std_ratio={"model": R}`: per-env stiffness and damping of every
+flexibility joint, re-drawn at every restart; r <= 2 on that robot).
+
+    python tools/bench_pipeline.py [--robot atlas|anymal|anymal_flexible] [--loop host|device] [--alternate R]
+                                   [--n-env 4096] [--steps 10] [--warmup 3] [--duration-max 0.4] [--disturbance R]
+                                   [--sensors R] [--model R]
 """
 import argparse
 import json
@@ -46,13 +51,13 @@ KEYS = [("states", "pd_controller"), ("measurements", "EncoderSensor"), ("featur
 
 
 def make_env(n_env: int, api_=None, robot: str = "atlas", loop: str = "host", duration_max: float = 20.0,
-             disturbance: float = 0.0, sensors: float = 0.0):
+             disturbance: float = 0.0, sensors: float = 0.0, model: float = 0.0):
     from jiminy_b200 import envs, scenarios
-    ratio = {k: r for k, r in (("disturbance", disturbance), ("sensors", sensors)) if r > 0}
+    ratio = {k: r for k, r in (("disturbance", disturbance), ("sensors", sensors), ("model", model)) if r > 0}
     kw = dict(simulation_duration_max=duration_max, api_=api_, std_ratio=ratio or None)
-    if robot == "anymal":
+    if robot in ("anymal", "anymal_flexible"):
         from jiminy_b200.torch_envs import DeviceBatchedEnv
-        return (DeviceBatchedEnv if loop == "device" else envs.BatchedJiminyEnv)(scenarios.make("anymal", n_env, seed=0), **kw)
+        return (DeviceBatchedEnv if loop == "device" else envs.BatchedJiminyEnv)(scenarios.make(robot, n_env, seed=0), **kw)
     from jiminy_b200.torch_envs import DevicePDControlBatchedEnv
     sc = scenarios.make(robot, n_env, seed=0, contact_model="constraint", solver="euler_explicit", dt_max=0.005)
     return (DevicePDControlBatchedEnv if loop == "device" else envs.PDControlBatchedEnv)(
@@ -82,15 +87,15 @@ def gpu_info() -> dict:
 
 
 def run(n_env: int, steps: int, warmup: int, api_=None, robot: str = "atlas", loop: str = "host",
-        duration_max: float = 0.4, disturbance: float = 0.0, sensors: float = 0.0) -> dict:
+        duration_max: float = 0.4, disturbance: float = 0.0, sensors: float = 0.0, model: float = 0.0) -> dict:
     import torch
     from jiminy_b200.envs import flatten_observation
-    env = make_env(n_env, api_, robot, loop, duration_max, disturbance, sensors)
+    env = make_env(n_env, api_, robot, loop, duration_max, disturbance, sensors, model)
     device = loop == "device"
     on_gpu = device and env.torch_device.type == "cuda"
     nm = env.robot.nmotors
     # the actions of the run, made before the clock starts (device loop: already on the device)
-    if robot == "anymal":
+    if robot != "atlas":
         acts = [env.sc.sample_targets(k) for k in range(warmup + steps)]
     else:
         acts = [np.zeros((n_env, nm))] * (warmup + steps)      # `env.action` after reset: target velocities = 0
@@ -126,9 +131,9 @@ def run(n_env: int, steps: int, warmup: int, api_=None, robot: str = "atlas", lo
     q = q.cpu().numpy() if hasattr(q, "cpu") else q
     desc = (f"{robot} PD-control pipeline (MotorSafetyLimit + PDController + PDAdapter(order=1) + MahonyFilter), constraint "
             f"contacts, euler_explicit 5 ms" if robot == "atlas" else
-            "anymal PD standing (plain PD law), spring-damper contacts, runge_kutta_4 1 ms, per-step position targets")
+            f"{robot} PD standing (plain PD law), spring-damper contacts, runge_kutta_4 1 ms, per-step position targets")
     out = {"metric": "env_steps_per_sec", "unit": "env-steps/s", "value": n_env * steps / dt, "ms_per_step": 1e3 * dt / steps,
-           "loop": loop, "robot": robot, "disturbance": disturbance, "sensors": sensors, "n_env": n_env, "steps": steps, "warmup": warmup,
+           "loop": loop, "robot": robot, "disturbance": disturbance, "sensors": sensors, "model": model, "n_env": n_env, "steps": steps, "warmup": warmup,
            "timing": "host clock around env.step + flatten_observation, ending in a device synchronise",
            "config": {"workload": f"{desc}, {n_env} envs, step_dt {env.step_dt}, simulation_duration_max {duration_max}",
                       "env": type(env).__name__, "lane_plan": env.engine.describe(), "observation_width": int(flat.shape[1])},
@@ -158,7 +163,7 @@ def alternate(rounds: int, **kw) -> dict:
 
 
 def alternate_randomisation(rounds: int, ratios: dict, loops, **kw) -> dict:
-    """Each loop with the randomisation of `ratios` ({"disturbance": r} and / or {"sensors": r}) off and on, `rounds`
+    """Each loop with the randomisation of `ratios` ({"disturbance": r}, {"sensors": r}, {"model": r}) off and on, `rounds`
     times in this process, alternating; env-steps/s and spread."""
     name = "_".join(ratios)
     runs = {(loop, on): [] for loop in loops for on in (False, True)}
@@ -184,14 +189,15 @@ if __name__ == "__main__":
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--loop", choices=("host", "device"), default="host")
-    ap.add_argument("--robot", choices=("atlas", "anymal"), default="atlas")
+    ap.add_argument("--robot", choices=("atlas", "anymal", "anymal_flexible"), default="atlas")
     ap.add_argument("--alternate", type=int, default=0, metavar="R")
     ap.add_argument("--duration-max", type=float, default=0.4)
     ap.add_argument("--disturbance", type=float, default=0.0, metavar="R")
     ap.add_argument("--sensors", type=float, default=0.0, metavar="R")
+    ap.add_argument("--model", type=float, default=0.0, metavar="R")
     a = ap.parse_args()
     kw = dict(n_env=a.n_env, steps=a.steps, warmup=a.warmup, robot=a.robot, duration_max=a.duration_max)
-    ratios = {k: r for k, r in (("disturbance", a.disturbance), ("sensors", a.sensors)) if r > 0}
+    ratios = {k: r for k, r in (("disturbance", a.disturbance), ("sensors", a.sensors), ("model", a.model)) if r > 0}
     if ratios:
         res = alternate_randomisation(max(a.alternate, 1), ratios, ("host", "device") if a.alternate > 0 else (a.loop,), **kw)
     else:
