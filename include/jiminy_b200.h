@@ -223,6 +223,13 @@ int jb_start(JbBatch* batch, const uint8_t* mask, const double* q0, const double
  * JB_ENV_BAD_START and nothing else of it is written -- while the other envs start normally.  The generator start
  * states of the sensor pipeline are recomputed on the host only after jb_set_seeds / jb_set_sensor_options. */
 int jb_start_device(JbBatch* batch, const uint8_t* mask_dev, const double* q0_dev, const double* v0_dev);
+/* jb_start_device that first puts every started env on the ground: before the input checks, the kernel sets
+ * q[2] -= min_i z_i, where z_i is the world height of contact frame i by forward kinematics of the env's own row (its
+ * block's model variant included).  This is the rule of BaseJiminyEnv._sample_state (generic.py:1300-1335) as the host
+ * envs apply it (robots.ground_base_height): a z shift of the free-flyer onto flat ground, orientation untouched.  The
+ * caller's buffers are not written.  A row with a NaN still ends JB_ENV_NOT_STARTED | JB_ENV_BAD_START.  On a model
+ * without a free-flyer or without a contact frame the call is jb_start_device. */
+int jb_start_device_on_ground(JbBatch* batch, const uint8_t* mask_dev, const double* q0_dev, const double* v0_dev);
 
 /* Replaces: the command buffer written by AbstractController::computeCommand through the
  * FunctionalController callback (engine.cc:3240-3251; controller_functor.h:27-80).  The command is

@@ -64,7 +64,7 @@ class Api:
                "jb_get_pd_controller_state", "jb_set_pd_controller_state", "jb_get_constraints",
                "jb_get_stepper_state", "jb_set_stepper_state", "jb_get_centroidal",
                "jb_set_sensor_options", "jb_set_seeds", "jb_get_sensor_data",
-               "jb_start_device", "jb_set_pd_adapter", "jb_pd_adapter_device", "jb_device_block_views",
+               "jb_start_device", "jb_start_device_on_ground", "jb_set_pd_adapter", "jb_pd_adapter_device", "jb_device_block_views",
                "jb_set_impulse_force_device", "jb_register_process_force", "jb_set_process_force",
                "jb_set_process_force_device", "jb_enable_per_env_sensor_options", "jb_set_sensor_options_env",
                "jb_set_sensor_options_env_device", "jb_set_seeds_device",
@@ -133,6 +133,7 @@ class Api:
         L.jb_peer_obs_enable.argtypes = [vp, C.c_int32]
         L.jb_peer_obs_view.argtypes = [vp, C.POINTER(vp)]
         L.jb_start_device.argtypes = [vp, vp, vp, vp]
+        L.jb_start_device_on_ground.argtypes = [vp, vp, vp, vp]
         L.jb_set_pd_adapter.argtypes = [vp, C.c_int32, C.c_int32, c_double_p]
         L.jb_pd_adapter_device.argtypes = [vp, vp, C.c_double]
         L.jb_device_block_views.argtypes = [vp, C.POINTER(vp), C.POINTER(vp), C.POINTER(vp)]
@@ -440,12 +441,14 @@ class BatchedEngine:
         self._api.check(self._api.dll.jb_start(self._h, None if m is None else m.ctypes.data_as(c_uint8_p),
                                                dptr(q0), dptr(v0)))
 
-    def start_device(self, q0_ptr: int, v0_ptr: int, mask_ptr: Optional[int] = None) -> None:
+    def start_device(self, q0_ptr: int, v0_ptr: int, mask_ptr: Optional[int] = None, on_ground: bool = False) -> None:
         """`start` from device buffers (q0 [n_env, nq], v0 [n_env, nv] fp64, mask [n_env] uint8 or None = all), enqueued on
         the batch stream with no host synchronisation: keep the buffers alive until the stream has passed the call.  Rows
-        that fail the input checks leave their env not started, with status JB_ENV_NOT_STARTED | JB_ENV_BAD_START."""
-        self._api.check(self._api.dll.jb_start_device(self._h, C.c_void_p(mask_ptr or None), C.c_void_p(q0_ptr),
-                                                      C.c_void_p(v0_ptr)))
+        that fail the input checks leave their env not started, with status JB_ENV_NOT_STARTED | JB_ENV_BAD_START.
+        `on_ground`: each started env's free-flyer height is first shifted so that its lowest contact frame touches z = 0
+        (`robots.ground_base_height` in the kernel, `jb_start_device_on_ground`); the buffers are not written."""
+        fn = self._api.dll.jb_start_device_on_ground if on_ground else self._api.dll.jb_start_device
+        self._api.check(fn(self._h, C.c_void_p(mask_ptr or None), C.c_void_p(q0_ptr), C.c_void_p(v0_ptr)))
 
     def set_pd_adapter(self, order: int = 1, is_instantaneous: bool = False, velocity_deadband=None) -> None:
         """Configures the device `PDAdapter` block in front of the `PDController` block (`set_pd_controller_full`)."""

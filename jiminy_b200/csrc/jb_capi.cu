@@ -221,13 +221,14 @@ static bool forces_on_hot_path(const JbBatch* b) {
            kp.opt.ode_solver != JB_SOLVER_RUNGE_KUTTA_DOPRI && !b->no_fast_kernel;
 }
 static int launch(JbBatch* b, int mode, double step_dt, const uint8_t* d_mask = nullptr, const double* d_command = nullptr,
-                  bool validate = false) {
+                  bool validate = false, bool ground = false) {
     KParams kp = b->kp;
     // the static plan signatures of the full body carry no external-force code (the force-carrying hot path knows its
     // signature at compile time)
     if (kp.n_eslot > 0) kp.sig_id = 0;
     LaunchArgs la{};
     la.mode = mode; la.step_dt = step_dt; la.mask = d_mask; la.command = d_command; la.validate = validate ? 1 : 0;
+    la.ground = ground ? 1 : 0;
     if (mode == MODE_STEP && b->peer_world > 1 && !b->peer_opened.empty() && b->peer_enabled) {
         ++b->step_id;
         la.peer_on = 1;
@@ -1451,7 +1452,7 @@ int jb_start(JbBatch* b, const uint8_t* mask, const double* q0, const double* v0
     return JB_OK;
 }
 
-int jb_start_device(JbBatch* b, const uint8_t* mask_dev, const double* q0_dev, const double* v0_dev) {
+static int start_device(JbBatch* b, const uint8_t* mask_dev, const double* q0_dev, const double* v0_dev, bool ground) {
     if (!b || !q0_dev || !v0_dev) return fail(JB_ERR_INVALID_ARGUMENT, "null argument");
     CU(cudaSetDevice(b->device));
     CU(cudaMemcpyAsync(b->d_qin, q0_dev, sizeof(double) * b->n_env * b->nq, cudaMemcpyDeviceToDevice, b->stream));
@@ -1460,10 +1461,19 @@ int jb_start_device(JbBatch* b, const uint8_t* mask_dev, const double* q0_dev, c
     int rc = prepare_sensor_pipeline(b, nullptr, true);
     if (rc) return rc;
     // the input checks run in the kernel (LaunchArgs::validate): no decision here depends on device data
-    rc = launch(b, MODE_START, 0.0, mask_dev ? b->d_mask : nullptr, nullptr, true);
+    rc = launch(b, MODE_START, 0.0, mask_dev ? b->d_mask : nullptr, nullptr, true, ground);
     if (rc) return rc;
     b->any_started = true;
     return JB_OK;
+}
+
+int jb_start_device(JbBatch* b, const uint8_t* mask_dev, const double* q0_dev, const double* v0_dev) {
+    return start_device(b, mask_dev, q0_dev, v0_dev, false);
+}
+
+// the rows are copied into the batch's own input buffer first, so the kernel places that copy, never the caller's rows
+int jb_start_device_on_ground(JbBatch* b, const uint8_t* mask_dev, const double* q0_dev, const double* v0_dev) {
+    return start_device(b, mask_dev, q0_dev, v0_dev, true);
 }
 
 // ---- external forces --------------------------------------------------------------------------

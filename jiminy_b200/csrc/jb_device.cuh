@@ -38,6 +38,7 @@ struct LaunchArgs {
     double step_dt;
     const uint8_t* mask;           // MODE_START: envs to (re)start, null = all
     const double* command;         // MODE_DYNAMICS: the command of this evaluation (the held command of the running envs is not touched)
+    int32_t ground;                // MODE_START from device inputs: each started env's free-flyer height is placed first (place_on_ground)
 };
 
 // One sensor of the measurement pipeline (AbstractSensorOptions, core/include/jiminy/core/hardware/abstract_sensor.h:66-100)
@@ -856,6 +857,58 @@ JB_DI const double* flex_params(const Ctx& c, int r, int L, const RecDbl* rd) {
         return rd->motor;
 }
 
+// Joint transform of a record at its stage state (JointModel*::calc of Pinocchio 2.7): liMi, the joint velocity vJ and,
+// for one-dof joints, qd (the caller zeroes vJ and qd).  P: the record's placement, ax its axis, rp its smem base.  One
+// routine for the forward sweep (rhs_impl) and the ground placement of a start (place_on_ground).
+JB_DI void joint_calc(const Ctx& c, const int kind, const double* P, const V3 ax, double* const rp, const int base,
+                      Xf& li, Mot& vJ, double& qd) {
+    if (kind == REC_FREE) {
+        double Rq[9];
+        quat_to_R(RP(RF_QS + 3), RP(RF_QS + 4), RP(RF_QS + 5), RP(RF_QS + 6), Rq);
+        mat3mul(P, Rq, li.R);
+        li.p = ld3(P + 9) + rmul(P, mk(RP(RF_QS), RP(RF_QS + 1), RP(RF_QS + 2)));
+        vJ = sm_load_mot(c, base + RF_VS);
+    } else if (kind == REC_SPH) {
+        // JointModelSphericalTpl::calc: M = (quat.matrix(), 0), v = (0, omega)
+        double Rq[9];
+        quat_to_R(RP(RF_QS + 3), RP(RF_QS + 4), RP(RF_QS + 5), RP(RF_QS + 6), Rq);
+        mat3mul(P, Rq, li.R);
+        li.p = ld3(P + 9);
+        vJ.a = mk(RP(RF_VS + 3), RP(RF_VS + 4), RP(RF_VS + 5));
+    } else if (kind == REC_PRISM) {
+#pragma unroll
+        for (int k = 0; k < 9; ++k) li.R[k] = P[k];
+        li.p = ld3(P + 9) + rmul(P, RP(R1_QS) * ax);
+        qd = RP(R1_VS);
+        vJ.l = qd * ax;
+    } else if (kind == REC_REVX) {
+        // revolute about +-x of the joint frame (JointModelRX, or RevoluteUnaligned with axis -x):
+        // liMi.R = Rp Rx(+-q) touches two columns only
+        double ca, sa;
+        sincos(RP(R1_QS), &sa, &ca);
+        const double s = ax.x * sa;
+#pragma unroll
+        for (int i = 0; i < 3; ++i) {
+            li.R[3 * i] = P[3 * i];
+            li.R[3 * i + 1] = ca * P[3 * i + 1] + s * P[3 * i + 2];
+            li.R[3 * i + 2] = ca * P[3 * i + 2] - s * P[3 * i + 1];
+        }
+        li.p = ld3(P + 9);
+        qd = RP(R1_VS);
+        vJ.a = mk(ax.x * qd, 0.0, 0.0);
+    } else {
+        double ca, sa;
+        if (kind == REC_REVU) { ca = RP(R1_QS); sa = RP(R1_QS + 1); }
+        else sincos(RP(R1_QS), &sa, &ca);
+        double Rj[9];
+        axis_angle_R(ax, ca, sa, Rj);
+        mat3mul(P, Rj, li.R);
+        li.p = ld3(P + 9);
+        qd = RP(R1_VS);
+        vJ.a = qd * ax;
+    }
+}
+
 template <class SIG>
 JB_DI bool rhs_impl(const Ctx c, const bool up_to_date, int* status) {
     const int L = SIG::lanes();
@@ -890,51 +943,7 @@ JB_DI bool rhs_impl(const Ctx c, const bool up_to_date, int* status) {
             Xf li; Mot vJ = mzero();
             const V3 ax = ld3(K.axis);
             double qd = 0.0;
-            if (kind == REC_FREE) {
-                double Rq[9];
-                quat_to_R(RP(RF_QS + 3), RP(RF_QS + 4), RP(RF_QS + 5), RP(RF_QS + 6), Rq);
-                mat3mul(K.placement, Rq, li.R);
-                li.p = ld3(K.placement + 9) + rmul(K.placement, mk(RP(RF_QS), RP(RF_QS + 1), RP(RF_QS + 2)));
-                vJ = sm_load_mot(c, base + RF_VS);
-            } else if (kind == REC_SPH) {
-                // JointModelSphericalTpl::calc: M = (quat.matrix(), 0), v = (0, omega)
-                double Rq[9];
-                quat_to_R(RP(RF_QS + 3), RP(RF_QS + 4), RP(RF_QS + 5), RP(RF_QS + 6), Rq);
-                mat3mul(K.placement, Rq, li.R);
-                li.p = ld3(K.placement + 9);
-                vJ.a = mk(RP(RF_VS + 3), RP(RF_VS + 4), RP(RF_VS + 5));
-            } else if (kind == REC_PRISM) {
-#pragma unroll
-                for (int k = 0; k < 9; ++k) li.R[k] = K.placement[k];
-                li.p = ld3(K.placement + 9) + rmul(K.placement, RP(R1_QS) * ax);
-                qd = RP(R1_VS);
-                vJ.l = qd * ax;
-            } else if (kind == REC_REVX) {
-                // revolute about +-x of the joint frame (JointModelRX, or RevoluteUnaligned with axis -x):
-                // liMi.R = Rp Rx(+-q) touches two columns only
-                double ca, sa;
-                sincos(RP(R1_QS), &sa, &ca);
-                const double s = ax.x * sa;
-#pragma unroll
-                for (int i = 0; i < 3; ++i) {
-                    li.R[3 * i] = K.placement[3 * i];
-                    li.R[3 * i + 1] = ca * K.placement[3 * i + 1] + s * K.placement[3 * i + 2];
-                    li.R[3 * i + 2] = ca * K.placement[3 * i + 2] - s * K.placement[3 * i + 1];
-                }
-                li.p = ld3(K.placement + 9);
-                qd = RP(R1_VS);
-                vJ.a = mk(ax.x * qd, 0.0, 0.0);
-            } else {
-                double ca, sa;
-                if (kind == REC_REVU) { ca = RP(R1_QS); sa = RP(R1_QS + 1); }
-                else sincos(RP(R1_QS), &sa, &ca);
-                double Rj[9];
-                axis_angle_R(ax, ca, sa, Rj);
-                mat3mul(K.placement, Rj, li.R);
-                li.p = ld3(K.placement + 9);
-                qd = RP(R1_VS);
-                vJ.a = qd * ax;
-            }
+            joint_calc(c, kind, K.placement, ax, rp, base, li, vJ, qd);
             // oMi = oMi[parent] * liMi ; v = vJ + liMi.actInv(v[parent]) ; a_gf bias = v x vJ (c == 0 for
             // every supported joint).  A child of the universe has oMi = liMi, v = vJ, bias = 0.
             Xf oM; Mot v, bias;

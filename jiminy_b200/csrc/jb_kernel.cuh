@@ -78,6 +78,65 @@ JB_DI void normalize_record(const Ctx& c, const RecInt* ri, int base) {
     }
 }
 
+// jb_start_device_on_ground: `robots.ground_base_height` on the device (the rule of BaseJiminyEnv._sample_state,
+// generic.py:1300-1335): q[2] of this env's input row is lowered or raised so that its lowest contact frame touches the
+// flat ground z = 0.  The forward kinematics runs on the row as given (before the start's quaternion normalisation), with
+// the forward sweep's joint transforms (joint_calc) and this block's model variant.  Each lane takes the min over its own
+// contact slots, then every lane reads the group's lane minima in the order 0 .. L-1, so that all of them agree bit for
+// bit.  Sub-lane 0 writes q[2] into the batch's own copy of the row (KP->q_in), which the input checks and the loads of
+// the start then read.  The min keeps a NaN, so a row that yields one still fails the checks.  Without a free-flyer at
+// q[0:7] or without a contact frame the row is left as it is.
+__device__ __noinline__ void place_on_ground(const Ctx c) {
+    const int L = KP->L;
+    bool has_free = false;
+    for (int r = 0; r < KP->nrec; ++r) {
+        const RecInt* ri = KP->rint + (r * L + c.sub);
+        if (ri->kind == REC_PAD) continue;
+        load_record_state_aos(c, ri, KP->rec_off[r], KP->q_in, KP->v_in, c.env);
+        has_free = has_free || (ri->kind == REC_FREE && ri->idx_q == 0);
+    }
+    stage_from_accepted(c);
+    double zmin = D_INF;
+    bool any_contact = false;
+    Xf oMc;
+#pragma unroll
+    for (int k = 0; k < 9; ++k) oMc.R[k] = 0.0;
+    oMc.p = mk(0, 0, 0);
+    for (int r = 0; r < KP->nrec; ++r) {
+        const RecInt* ri = KP->rint + (r * L + c.sub);
+        if (ri->kind == REC_PAD) continue;
+        const RecDbl* rd = JB_RDBL + (r * L + c.sub);
+        const int base = KP->rec_off[r];
+        double* const rp = jb_smem + base * 32 + c.lane;
+        if (ri->parent_rec >= 0 && !ri->carry_in) sm_load_xf(c, KP->pool_off + POOL_SIZE * ri->parent_pool, oMc);
+        Xf li; Mot vJ = mzero();
+        double qd = 0.0;
+        joint_calc(c, ri->kind, rd->placement, ld3(rd->axis), rp, base, li, vJ, qd);
+        Xf oM;
+        if (ri->parent_rec < 0) oM = li;
+        else {
+            mat3mul(oMc.R, li.R, oM.R);
+            oM.p = oMc.p + rmul(oMc.R, li.p);
+        }
+        for (int k = 0; k < ri->ncontact; ++k) {
+            const ContactSlot* ct = KP->cslots + ((ri->contact0 + k) * L + c.sub);
+            const double z = (oM.p + rmul(oM.R, ld3(ct->placement + 9))).z;
+            zmin = (z < zmin || z != z) ? z : zmin;
+            any_contact = true;
+        }
+        if (ri->pool >= 0) sm_store_xf(c, KP->pool_off + POOL_SIZE * ri->pool, oM);
+        oMc = oM;
+    }
+    double zg = D_INF;
+    for (int k = 0; k < L; ++k) {
+        const double z = jb_shfl(c, zmin, c.lane - c.sub + k);
+        zg = (z < zg || z != z) ? z : zg;
+    }
+    if (jb_any(c, has_free) && jb_any(c, any_contact) && c.valid && c.sub == 0)
+        const_cast<double*>(KP->q_in)[static_cast<size_t>(c.env) * KP->nq + 2] -= zg;
+    jb_syncwarp(c);
+}
+
 // Device-side controller block: gym_jiminy.common.blocks.pd_controller
 // (python/gym_jiminy/common/gym_jiminy/common/blocks/proportional_derivative_controller.py:101-165)
 // for a zero-order-held position target and zero target velocity,
@@ -391,6 +450,7 @@ __device__ __forceinline__ void env_step_body(const LaunchArgs& la, const bool o
     const bool masked_out = (mode == MODE_START) && la.mask != nullptr && la.mask[c.env] == 0;
     if (masked_out) return;   // whole env (all its lanes) leaves: group masks keep the others safe
     if constexpr (!FAST) {
+        if (mode == MODE_START && la.ground) place_on_ground(c);
         // jb_start_device: the input checks jb_start runs on the host (Engine::start, engine.cc:1007-1037), per env.  An env
         // whose row fails them is not started and writes nothing but its status word.
         if (mode == MODE_START && la.validate) {

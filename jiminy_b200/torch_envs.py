@@ -13,10 +13,14 @@ What differs from the host envs is only where the work runs:
   tensor: envs outside the mask leave at the top of the launch, so no host decision depends on device data.
 
 Restart states.  The host env draws a fresh sample of the scenario's initial-state distribution at every restart event
-(`scenarios.make`: a perturbed posture with the feet put on the ground by forward kinematics on the host).  Here the
-restart rows are drawn on the device, with replacement, from a fixed bank `reset_states=(q [B, nq], v [B, nv])`; the
+(`scenarios.make`: a perturbed posture with the feet put on the ground by forward kinematics on the host).  By default
+the restart rows are drawn on the device, with replacement, from a fixed bank `reset_states=(q [B, nq], v [B, nv])`; the
 default bank is one such sample of `n_env` rows.  The bank is validated once on the host.  `info["reset_rows"]` gives the
 bank row each env restarted from (-1: not restarted).  This is the one semantic difference from the host env.
+`reset_states="sample"` removes it: at every step `n_env` fresh rows of the distribution are drawn with the env's torch
+generator (`Scenario.draw_initial_torch`) and the masked restart is `jb_start_device_on_ground`, which puts each
+restarted env's feet on the ground by forward kinematics in the start kernel (`robots.ground_base_height` on the
+device).  There is no bank, so `info["reset_rows"]` is not returned; the next observation holds the placed states.
 
 Disturbance.  With `std_ratio={"disturbance": r}` the walker disturbance (`jiminy_b200.disturbance`) of the envs in the
 done mask is re-drawn with a torch generator on the device and written by the device setters before the masked restart,
@@ -45,7 +49,7 @@ from __future__ import annotations
 
 import contextlib
 import ctypes as C
-from typing import Any, Dict, Optional, Tuple
+from typing import Any, Dict, Optional, Tuple, Union
 
 import numpy as np
 import torch
@@ -72,10 +76,10 @@ def validate_reset_states(robot, q: np.ndarray, v: np.ndarray) -> None:
 
 class DeviceBatchedEnv(envs.BatchedJiminyEnv):
     """`BatchedJiminyEnv` with torch actions and observations on the batch's device and the restart on the device.
-    Extra arguments: `reset_states` (restart bank, see the module docstring) and `torch_device` (default: cuda:<device>,
-    or cpu with the emulated library)."""
+    Extra arguments: `reset_states` (restart bank, or "sample" for fresh grounded draws: see the module docstring) and
+    `torch_device` (default: cuda:<device>, or cpu with the emulated library)."""
 
-    def __init__(self, scenario: scenarios.Scenario, reset_states: Optional[Tuple[np.ndarray, np.ndarray]] = None,
+    def __init__(self, scenario: scenarios.Scenario, reset_states: Union[None, str, Tuple[np.ndarray, np.ndarray]] = None,
                  torch_device=None, **kw):
         super().__init__(scenario, **kw)
         self._init_device(reset_states, torch_device, kw.get("api_"))
@@ -90,14 +94,20 @@ class DeviceBatchedEnv(envs.BatchedJiminyEnv):
         self._stream = None if self._emulated else torch.cuda.ExternalStream(eng.stream(), device=dev)
         # the default bank: one sample of the distribution the host env's `_sample_state` draws from
         seed = int(np.random.default_rng([self.sc.seed, 0x5EED]).integers(0, 2 ** 31 - 1))
-        if reset_states is None:
-            bank = scenarios.make(self.sc.name, n, seed=seed)
-            reset_states = (bank.q0, bank.v0)
-        q_bank = np.ascontiguousarray(reset_states[0], dtype=np.float64)
-        v_bank = np.ascontiguousarray(reset_states[1], dtype=np.float64)
-        validate_reset_states(self.robot, q_bank, v_bank)
         f64 = dict(dtype=torch.float64, device=dev)
-        self.reset_states = (torch.as_tensor(q_bank, **f64), torch.as_tensor(v_bank, **f64))
+        self._sample_restarts = isinstance(reset_states, str)
+        if self._sample_restarts:
+            if reset_states != "sample":
+                raise ValueError(f"reset_states must be None, 'sample' or (q, v), not {reset_states!r}")
+            self.reset_states = None
+        else:
+            if reset_states is None:
+                bank = scenarios.make(self.sc.name, n, seed=seed)
+                reset_states = (bank.q0, bank.v0)
+            q_bank = np.ascontiguousarray(reset_states[0], dtype=np.float64)
+            v_bank = np.ascontiguousarray(reset_states[1], dtype=np.float64)
+            validate_reset_states(self.robot, q_bank, v_bank)
+            self.reset_states = (torch.as_tensor(q_bank, **f64), torch.as_tensor(v_bank, **f64))
         self._gen = torch.Generator(device=dev)
         self._gen.manual_seed(seed)
         # inputs of the launches, kept alive between steps (every use is ordered on the batch stream)
@@ -228,24 +238,33 @@ class DeviceBatchedEnv(envs.BatchedJiminyEnv):
         self.model_rows.copy_(new if done is None else torch.where(done.view(-1, 1, 1), new, self.model_rows))
         self.model_randomisation.apply_device(self.engine, self.model_rows, None if done is None else self._mask.data_ptr())
 
-    def _restart(self, done: torch.Tensor) -> torch.Tensor:
-        """Masked restart of the envs in `done` from bank rows drawn on the device; returns the rows (-1: not restarted)."""
-        q_bank, v_bank = self.reset_states
-        rows = torch.randint(0, q_bank.shape[0], (self.n_env,), generator=self._gen, device=self.torch_device)
-        torch.index_select(q_bank, 0, rows, out=self._q_start)
-        torch.index_select(v_bank, 0, rows, out=self._v_start)
+    def _restart(self, done: torch.Tensor) -> Optional[torch.Tensor]:
+        """Masked restart of the envs in `done` from bank rows drawn on the device; returns the rows (-1: not restarted).
+        With `reset_states="sample"`: from fresh draws put on the ground in the start kernel; returns None."""
+        if self._sample_restarts:
+            q, v = self.sc.draw_initial_torch(self._gen, self.n_env, self.torch_device)
+            self._q_start.copy_(q)
+            self._v_start.copy_(v)
+            rows = None
+        else:
+            q_bank, v_bank = self.reset_states
+            rows = torch.randint(0, q_bank.shape[0], (self.n_env,), generator=self._gen, device=self.torch_device)
+            torch.index_select(q_bank, 0, rows, out=self._q_start)
+            torch.index_select(v_bank, 0, rows, out=self._v_start)
         self._mask.copy_(done)
         self._redraw_disturbance(done)
         self._redraw_sensors(done)
         self._redraw_model(done)
-        self.engine.start_device(self._q_start.data_ptr(), self._v_start.data_ptr(), self._mask.data_ptr())
+        self.engine.start_device(self._q_start.data_ptr(), self._v_start.data_ptr(), self._mask.data_ptr(),
+                                 on_ground=self._sample_restarts)
         self.num_steps.masked_fill_(done, 0)
-        return torch.where(done, rows, torch.full_like(rows, -1))
+        return None if rows is None else torch.where(done, rows, torch.full_like(rows, -1))
 
     # ------------------------------------------------------------------ gym API
     def reset(self, mask: Optional[torch.Tensor] = None) -> Tuple[Dict[str, Any], Dict[str, Any]]:
         """First call (or `mask=None`): every env starts -- from the scenario's initial states the first time, from bank
-        rows afterwards.  `mask` [n_env] (bool / uint8 tensor): a masked restart of those envs from bank rows."""
+        rows (or fresh grounded draws) afterwards.  `mask` [n_env] (bool / uint8 tensor): a masked restart of those envs
+        the same way."""
         with self._on_batch_stream() as caller:
             info: Dict[str, Any] = {}
             if not self._started:
@@ -261,7 +280,9 @@ class DeviceBatchedEnv(envs.BatchedJiminyEnv):
                     self._first_command()
                 done = torch.ones(self.n_env, dtype=torch.bool, device=self.torch_device) if mask is None else \
                     torch.as_tensor(mask, device=self.torch_device).to(torch.bool)
-                info["reset_rows"] = self._restart(done)
+                rows = self._restart(done)
+                if rows is not None:
+                    info["reset_rows"] = rows
             obs = self._observation()
             self._hand_over(caller, list(self._leaves(obs)) + list(info.values()))
         return obs, info
@@ -288,10 +309,12 @@ class DeviceBatchedEnv(envs.BatchedJiminyEnv):
             reward = (~terminated).to(torch.float64)             # SurviveReward
             done = terminated | truncated
             rows = self._restart(done)                           # enqueued at every step: no host decision
-            info = {"status": status, "final_observation": obs, "_final_observation": done, "reset_rows": rows}
+            info = {"status": status, "final_observation": obs, "_final_observation": done}
+            if rows is not None:
+                info["reset_rows"] = rows
             obs = self._observation()
             self._hand_over(caller, list(self._leaves(obs)) + list(self._leaves(info["final_observation"])) +
-                            [status, done, rows, reward, terminated, truncated])
+                            [status, done, reward, terminated, truncated] + ([] if rows is None else [rows]))
         return obs, reward, terminated, truncated, info
 
 

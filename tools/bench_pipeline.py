@@ -29,9 +29,13 @@ and jitter of every sensor and fresh generator seeds, re-drawn at every restart)
 turns the walker model randomisation on the same way (`std_ratio={"model": R}`: per-env stiffness and damping of every
 flexibility joint, re-drawn at every restart; r <= 2 on that robot).
 
+`--restart sample` times the device loop with its restarts from fresh draws of the initial-state distribution put on the
+ground in the start kernel (`reset_states="sample"`) against the default restart bank, alternating in one process,
+`max(--alternate, 1)` rounds; randomisation options given with it are on in both.
+
     python tools/bench_pipeline.py [--robot atlas|anymal|anymal_flexible] [--loop host|device] [--alternate R]
                                    [--n-env 4096] [--steps 10] [--warmup 3] [--duration-max 0.4] [--disturbance R]
-                                   [--sensors R] [--model R]
+                                   [--sensors R] [--model R] [--restart bank|sample]
 """
 import argparse
 import json
@@ -51,10 +55,14 @@ KEYS = [("states", "pd_controller"), ("measurements", "EncoderSensor"), ("featur
 
 
 def make_env(n_env: int, api_=None, robot: str = "atlas", loop: str = "host", duration_max: float = 20.0,
-             disturbance: float = 0.0, sensors: float = 0.0, model: float = 0.0):
+             disturbance: float = 0.0, sensors: float = 0.0, model: float = 0.0, restart: str = "bank"):
     from jiminy_b200 import envs, scenarios
     ratio = {k: r for k, r in (("disturbance", disturbance), ("sensors", sensors), ("model", model)) if r > 0}
     kw = dict(simulation_duration_max=duration_max, api_=api_, std_ratio=ratio or None)
+    if restart == "sample":
+        if loop != "device":
+            raise ValueError("--restart sample is an option of the device loop")
+        kw["reset_states"] = "sample"
     if robot in ("anymal", "anymal_flexible"):
         from jiminy_b200.torch_envs import DeviceBatchedEnv
         return (DeviceBatchedEnv if loop == "device" else envs.BatchedJiminyEnv)(scenarios.make(robot, n_env, seed=0), **kw)
@@ -87,10 +95,11 @@ def gpu_info() -> dict:
 
 
 def run(n_env: int, steps: int, warmup: int, api_=None, robot: str = "atlas", loop: str = "host",
-        duration_max: float = 0.4, disturbance: float = 0.0, sensors: float = 0.0, model: float = 0.0) -> dict:
+        duration_max: float = 0.4, disturbance: float = 0.0, sensors: float = 0.0, model: float = 0.0,
+        restart: str = "bank") -> dict:
     import torch
     from jiminy_b200.envs import flatten_observation
-    env = make_env(n_env, api_, robot, loop, duration_max, disturbance, sensors, model)
+    env = make_env(n_env, api_, robot, loop, duration_max, disturbance, sensors, model, restart)
     device = loop == "device"
     on_gpu = device and env.torch_device.type == "cuda"
     nm = env.robot.nmotors
@@ -133,7 +142,7 @@ def run(n_env: int, steps: int, warmup: int, api_=None, robot: str = "atlas", lo
             f"contacts, euler_explicit 5 ms" if robot == "atlas" else
             f"{robot} PD standing (plain PD law), spring-damper contacts, runge_kutta_4 1 ms, per-step position targets")
     out = {"metric": "env_steps_per_sec", "unit": "env-steps/s", "value": n_env * steps / dt, "ms_per_step": 1e3 * dt / steps,
-           "loop": loop, "robot": robot, "disturbance": disturbance, "sensors": sensors, "model": model, "n_env": n_env, "steps": steps, "warmup": warmup,
+           "loop": loop, "restart": restart, "robot": robot, "disturbance": disturbance, "sensors": sensors, "model": model, "n_env": n_env, "steps": steps, "warmup": warmup,
            "timing": "host clock around env.step + flatten_observation, ending in a device synchronise",
            "config": {"workload": f"{desc}, {n_env} envs, step_dt {env.step_dt}, simulation_duration_max {duration_max}",
                       "env": type(env).__name__, "lane_plan": env.engine.describe(), "observation_width": int(flat.shape[1])},
@@ -163,8 +172,8 @@ def alternate(rounds: int, **kw) -> dict:
 
 
 def alternate_randomisation(rounds: int, ratios: dict, loops, **kw) -> dict:
-    """Each loop with the randomisation of `ratios` ({"disturbance": r}, {"sensors": r}, {"model": r}) off and on, `rounds`
-    times in this process, alternating; env-steps/s and spread."""
+    """Each loop with the randomisation of `ratios` ({"disturbance": r}, {"sensors": r}, {"model": r}, or
+    {"restart": "sample"}) off and on, `rounds` times in this process, alternating; env-steps/s and spread."""
     name = "_".join(ratios)
     runs = {(loop, on): [] for loop in loops for on in (False, True)}
     for _ in range(rounds):
@@ -195,10 +204,13 @@ if __name__ == "__main__":
     ap.add_argument("--disturbance", type=float, default=0.0, metavar="R")
     ap.add_argument("--sensors", type=float, default=0.0, metavar="R")
     ap.add_argument("--model", type=float, default=0.0, metavar="R")
+    ap.add_argument("--restart", choices=("bank", "sample"), default="bank")
     a = ap.parse_args()
     kw = dict(n_env=a.n_env, steps=a.steps, warmup=a.warmup, robot=a.robot, duration_max=a.duration_max)
     ratios = {k: r for k, r in (("disturbance", a.disturbance), ("sensors", a.sensors), ("model", a.model)) if r > 0}
-    if ratios:
+    if a.restart == "sample":
+        res = alternate_randomisation(max(a.alternate, 1), {"restart": "sample"}, ("device",), **ratios, **kw)
+    elif ratios:
         res = alternate_randomisation(max(a.alternate, 1), ratios, ("host", "device") if a.alternate > 0 else (a.loop,), **kw)
     else:
         res = alternate(a.alternate, **kw) if a.alternate > 0 else run(loop=a.loop, **kw)
