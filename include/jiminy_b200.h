@@ -470,6 +470,29 @@ int jb_set_flexibility_env(JbBatch* batch, const uint8_t* mask, const double* ro
 int jb_set_flexibility_env_device(JbBatch* batch, const uint8_t* mask_dev, const double* rows_dev);
 int jb_get_flexibility_env(JbBatch* batch, double* out);
 
+/* Per-env model rows: the body biases of Model::addBiasedToExtendedModel (model.cc:1166-1236), which the reference
+ * re-draws at every reset (Model::reset -> generateModelExtended, model.cc:398-416), per env.
+ * jb_enable_per_env_model gives every env its own copy of the batch's double table and a pending row [njoints][13] in
+ * model joint order: per joint, mass, lever xyz, rotational inertia about the centre of mass (xx xy yy xz yz zz), joint-
+ * placement translation xyz.  Row 0 (the universe) is ignored.  Tables and rows start from each env's model values (its
+ * variant's with jb_set_model_variants, which is refused once this has run).  Refused (JB_ERR_INVALID_ARGUMENT) on a
+ * second call and when n_env times the rows of one table reaches 2^23.
+ * jb_set_model_env writes the pending rows [n_env][njoints][13] of the envs selected by mask (NULL = all).  Every start of
+ * an env expands its pending row into its table (every row of the joint, subtree masses and the total mass recomputed)
+ * before the start's grounding (jb_start_device_on_ground) and evaluations; a running env is not affected.  A row with a
+ * value that is not finite, or with a mass that is not positive (0 is accepted where the model's body is massless), is
+ * refused: the host form writes nothing and returns JB_ERR_INVALID_ARGUMENT naming the env; the _device form (device
+ * buffers, one kernel on the batch stream, no host synchronisation) skips that row and marks the env, whose starts then
+ * leave it JB_ENV_NOT_STARTED | JB_ENV_BAD_START until a valid row for it is written.  The mark is this setter's own.
+ * The expansion runs in a launch of its own ahead of the start kernel, for the started envs that no rejected device row
+ * (model rows, sensor options, flexibility parameters) refuses; an env whose start is refused by its input checks has
+ * still taken its pending row, which its next start takes again.
+ * jb_get_model_env reads the rows every env runs with (taken at its last start) [n_env][njoints][13]. */
+int jb_enable_per_env_model(JbBatch* batch);
+int jb_set_model_env(JbBatch* batch, const uint8_t* mask, const double* rows);
+int jb_set_model_env_device(JbBatch* batch, const uint8_t* mask_dev, const double* rows_dev);
+int jb_get_model_env(JbBatch* batch, double* out);
+
 /* Stable zero-copy views of the state, like the `StepperState` / `RobotState` members the reference exposes to Python as
  * array views of the engine's own memory (python/jiminy_pywrap/include/jiminy/python/functors.h:57-68, generic.py:688-690:
  * a gym env reads `q`, `v`, the sensor matrix every step without a getter call).  The first call with `host` non-null

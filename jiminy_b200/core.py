@@ -69,7 +69,8 @@ class Api:
                "jb_set_process_force_device", "jb_enable_per_env_sensor_options", "jb_set_sensor_options_env",
                "jb_set_sensor_options_env_device", "jb_set_seeds_device",
                "jb_enable_per_env_flexibility", "jb_set_flexibility_env", "jb_set_flexibility_env_device",
-               "jb_get_flexibility_env")
+               "jb_get_flexibility_env", "jb_enable_per_env_model", "jb_set_model_env", "jb_set_model_env_device",
+               "jb_get_model_env")
 
     def __init__(self, cdll: C.CDLL):
         self.dll = L = cdll
@@ -150,6 +151,10 @@ class Api:
         L.jb_set_flexibility_env.argtypes = [vp, c_uint8_p, c_double_p]
         L.jb_set_flexibility_env_device.argtypes = [vp, vp, vp]
         L.jb_get_flexibility_env.argtypes = [vp, c_double_p]
+        L.jb_enable_per_env_model.argtypes = [vp]
+        L.jb_set_model_env.argtypes = [vp, c_uint8_p, c_double_p]
+        L.jb_set_model_env_device.argtypes = [vp, vp, vp]
+        L.jb_get_model_env.argtypes = [vp, c_double_p]
 
     def check(self, rc: int) -> None:
         if rc != JB_OK:
@@ -586,6 +591,40 @@ class BatchedEngine:
         out = np.zeros((self.n_env, self.n_flex, 6))
         self._api.check(self._api.dll.jb_get_flexibility_env(self._h, dptr(out)))
         return out
+
+    # ---- per-env model rows (the body biases of the model options, re-drawn per env)
+    MODEL_ROW = 13
+
+    def enable_per_env_model(self) -> None:
+        """Per-env model rows (`set_model_env`): every env runs its own inertias and joint-placement translations,
+        starting from its model values.  Refused on a second call; `set_model_variants` is refused afterwards."""
+        self._api.check(self._api.dll.jb_enable_per_env_model(self._h))
+
+    def set_model_env(self, rows, mask: Optional[np.ndarray] = None) -> None:
+        """Rows [n_env, njoints, 13] (per joint: mass, lever xyz, inertia about the centre of mass xx xy yy xz yz zz,
+        joint-placement translation xyz; joint 0 ignored) of the envs of `mask` (None = all), applied from each env's
+        next start.  A value that is not finite or a mass that is not positive raises ValueError and nothing is
+        written."""
+        rows = self._per_env(rows, (self.robot.njoints, self.MODEL_ROW))
+        m = None if mask is None else np.ascontiguousarray(mask, dtype=np.uint8)
+        self._api.check(self._api.dll.jb_set_model_env(self._h, None if m is None else m.ctypes.data_as(c_uint8_p), dptr(rows)))
+
+    def set_model_env_device(self, rows_ptr: int, mask_ptr: Optional[int] = None) -> None:
+        """`set_model_env` from a device buffer of the same layout (fp64; mask [n_env] uint8 or None), enqueued on the
+        batch stream with no host synchronisation.  A rejected row is not written and its env stays
+        JB_ENV_NOT_STARTED | JB_ENV_BAD_START through its starts until a valid row for it arrives."""
+        self._api.check(self._api.dll.jb_set_model_env_device(self._h, C.c_void_p(mask_ptr or None), C.c_void_p(rows_ptr)))
+
+    def get_model_env(self) -> np.ndarray:
+        """The rows every env runs with (latched at its last start), [n_env, njoints, 13]."""
+        out = np.zeros((self.n_env, self.robot.njoints, self.MODEL_ROW))
+        self._api.check(self._api.dll.jb_get_model_env(self._h, dptr(out)))
+        return out
+
+    def model(self, env: int) -> "M.RobotTable":
+        """The robot table env `env` runs with: the batch's robot with that env's inertias and joint-placement
+        translations (`get_model_env`)."""
+        return M.with_body_rows(self.robot, self.get_model_env()[env])
 
     def get_sensor_data(self) -> np.ndarray:
         out = np.zeros((self.n_env, max(self.width, 1)))

@@ -125,6 +125,11 @@ struct JbBatch {
     // per-env flexibility parameters (jb_enable_per_env_flexibility): pending / active rows, host-setter staging, reject flags
     double *d_flex_pending = nullptr, *d_flex_active = nullptr, *d_flex_stage = nullptr;
     int32_t *d_flex_bad = nullptr, *d_flex_of_rec = nullptr;
+    // per-env model rows (jb_enable_per_env_model): parent of every joint, first (record, sub-lane) row of every joint
+    // (-1: none), 1 for the joints whose model mass is 0; pending rows, host-setter staging
+    std::vector<int32_t> h_joint_parent, h_pem_row, h_pem_massless;
+    double *d_pem_pending = nullptr, *d_pem_stage = nullptr;
+    int32_t* d_pem_massless = nullptr;
 };
 
 // The dynamic shared-memory opt-in is a per-function, per-device attribute: only ever raise it.
@@ -138,6 +143,10 @@ static int raise_smem_attr(int device, size_t bytes) {
     if (e == cudaSuccess) e = cudaFuncSetAttribute(env_step_kernel_t<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(bytes));
     if (e == cudaSuccess) e = cudaFuncSetAttribute(env_step_kernel_ext, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(bytes));
     if (e == cudaSuccess) e = cudaFuncSetAttribute(env_step_kernel_flex, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(bytes));
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(env_step_kernel_model_fast, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(bytes));
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(env_step_kernel_model_ext, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(bytes));
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(env_step_kernel_model, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(bytes));
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(env_step_kernel_model_flex, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(bytes));
     if (e != cudaSuccess) return fail(JB_ERR_CUDA, std::string("cudaFuncSetAttribute: ") + cudaGetErrorString(e));
     g_smem_attr[device] = bytes;
 #endif
@@ -220,6 +229,39 @@ static bool forces_on_hot_path(const JbBatch* b) {
     return kp.n_eslot > 0 && kp.sig_id == SigQuadruped::ID && kp.rhs_variant == 1 && kp.opt.contact_model == JB_CONTACT_SPRING_DAMPER &&
            kp.opt.ode_solver != JB_SOLVER_RUNGE_KUTTA_DOPRI && !b->no_fast_kernel;
 }
+// Per-env model rows (jb_enable_per_env_model): before a start, every started env's pending row becomes its table, one
+// thread per env, in a launch of its own so that the tables stay read-only inside every step-kernel launch (they are read
+// through the non-coherent cache).  Model::reset regenerates the biased model before Engine::reset (model.cc:398-416):
+// the start's grounding and evaluations see the env's own model.  Every (record, sub-lane) row of a joint takes its
+// inertia and placement translation (trunk rows: every lane); subtree masses and the total mass are summed over the tree
+// in build_plan's order (jb_plan.cpp), so that the model's own values give its bits.  Envs that the start refuses for a
+// rejected device row (model, sensor options, flexibility) keep their tables; an env refused by the start's input checks
+// has latched its row already, and its next start latches again.
+__global__ void latch_model_rows_kernel(RecDbl* __restrict__ tables, double* __restrict__ subtree, double* __restrict__ mass,
+                                        const double* __restrict__ pending, const RecInt* __restrict__ rint,
+                                        const int32_t* __restrict__ parent, const uint8_t* __restrict__ mask,
+                                        const int32_t* __restrict__ pem_bad, const int32_t* __restrict__ sp_bad,
+                                        const int32_t* __restrict__ flex_bad, int n_env, int nj, int nrows) {
+    const int e = blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= n_env || (mask && !mask[e])) return;
+    if (pem_bad[e] != 0 || (sp_bad && sp_bad[e] != 0) || (flex_bad && flex_bad[e] != 0)) return;
+    const double* const x = pending + static_cast<size_t>(e) * nj * PEM_W;
+    double* const sub = subtree + static_cast<size_t>(e) * nj;
+    sub[0] = 0.0;
+    for (int j = 1; j < nj; ++j) sub[j] = x[j * PEM_W];
+    for (int j = nj - 1; j > 0; --j) sub[parent[j]] += sub[j];
+    mass[e] = sub[0];
+    RecDbl* const t = tables + static_cast<size_t>(e) * nrows;
+    for (int i = 0; i < nrows; ++i) {
+        const RecInt& ri = rint[i];
+        if (ri.kind == REC_PAD) continue;
+        const double* xj = x + ri.joint * PEM_W;
+        for (int k = 0; k < 10; ++k) t[i].inertia[k] = xj[k];
+        for (int k = 0; k < 3; ++k) t[i].placement[9 + k] = xj[10 + k];
+        t[i].subtree_mass = sub[ri.joint];
+    }
+}
+
 static int launch(JbBatch* b, int mode, double step_dt, const uint8_t* d_mask = nullptr, const double* d_command = nullptr,
                   bool validate = false, bool ground = false) {
     KParams kp = b->kp;
@@ -236,16 +278,30 @@ static int launch(JbBatch* b, int mode, double step_dt, const uint8_t* d_mask = 
         la.peer_step = b->step_id;
     }
     // the hot-path kernel hands envs that leave the hot path over to the full body inside the same launch
-    // (per-env flexibility parameters: every launch runs env_step_kernel_flex)
+    // (per-env flexibility parameters: every launch runs env_step_kernel_flex; per-env model rows: the env_step_kernel_model
+    // instance of the kernel the same rules pick)
     const bool fast = mode == MODE_STEP && kp.n_eslot == 0 && kp.opt.contact_model == JB_CONTACT_SPRING_DAMPER &&
                       kp.opt.ode_solver != JB_SOLVER_RUNGE_KUTTA_DOPRI && !b->no_fast_kernel && !kp.flex_on;
     const bool fast_ext = mode == MODE_STEP && forces_on_hot_path(b);
     const int epw = 32 / b->plan.L;
     const int nblocks = (b->n_env + epw - 1) / epw;
+    if (mode == MODE_START && kp.pem_on) {
+        JB_LAUNCH(latch_model_rows_kernel, static_cast<unsigned>((b->n_env + 127) / 128), 128, 0, b->stream, kp.pem_rows, kp.pem_subtree,
+                  kp.pem_mass, kp.pem_pending, kp.rint, kp.pem_parent, d_mask, kp.pem_bad, kp.sp_env_on ? kp.sp_env_bad : nullptr,
+                  kp.flex_on ? kp.flex_bad : nullptr, b->n_env, kp.njoints, kp.rdbl_rows);
+        CU(cudaGetLastError());
+        ++b->launches;
+    }
 #ifdef JB_HOST_EMUL
     emul::current_L = b->plan.L;
     g_kp_host = kp;
-    if (kp.flex_on) JB_LAUNCH(env_step_kernel_flex, nblocks, 32, b->smem_bytes, b->stream, la);
+    if (kp.pem_on) {
+        if (kp.flex_on) JB_LAUNCH(env_step_kernel_model_flex, nblocks, 32, b->smem_bytes, b->stream, la);
+        else if (fast) JB_LAUNCH(env_step_kernel_model_fast, nblocks, 32, b->smem_bytes, b->stream, la);
+        else if (fast_ext) JB_LAUNCH(env_step_kernel_model_ext, nblocks, 32, b->smem_bytes, b->stream, la);
+        else JB_LAUNCH(env_step_kernel_model, nblocks, 32, b->smem_bytes, b->stream, la);
+    }
+    else if (kp.flex_on) JB_LAUNCH(env_step_kernel_flex, nblocks, 32, b->smem_bytes, b->stream, la);
     else if (fast) JB_LAUNCH(env_step_kernel_t<true>, nblocks, 32, b->smem_bytes, b->stream, la);
     else if (fast_ext) JB_LAUNCH(env_step_kernel_ext, nblocks, 32, b->smem_bytes, b->stream, la);
     else JB_LAUNCH(env_step_kernel_t<false>, nblocks, 32, b->smem_bytes, b->stream, la);
@@ -263,7 +319,13 @@ static int launch(JbBatch* b, int mode, double step_dt, const uint8_t* d_mask = 
             g_kp_valid[b->device] = true;
             ++b->param_uploads;
         }
-        if (kp.flex_on) JB_LAUNCH(env_step_kernel_flex, nblocks, 32, b->smem_bytes, b->stream, la);
+        if (kp.pem_on) {
+            if (kp.flex_on) JB_LAUNCH(env_step_kernel_model_flex, nblocks, 32, b->smem_bytes, b->stream, la);
+            else if (fast) JB_LAUNCH(env_step_kernel_model_fast, nblocks, 32, b->smem_bytes, b->stream, la);
+            else if (fast_ext) JB_LAUNCH(env_step_kernel_model_ext, nblocks, 32, b->smem_bytes, b->stream, la);
+            else JB_LAUNCH(env_step_kernel_model, nblocks, 32, b->smem_bytes, b->stream, la);
+        }
+        else if (kp.flex_on) JB_LAUNCH(env_step_kernel_flex, nblocks, 32, b->smem_bytes, b->stream, la);
         else if (fast) JB_LAUNCH(env_step_kernel_t<true>, nblocks, 32, b->smem_bytes, b->stream, la);
         else if (fast_ext) JB_LAUNCH(env_step_kernel_ext, nblocks, 32, b->smem_bytes, b->stream, la);
         else JB_LAUNCH(env_step_kernel_t<false>, nblocks, 32, b->smem_bytes, b->stream, la);
@@ -483,6 +545,7 @@ int jb_batch_create(const JbModelDesc* m, const JbOptions* opt, int32_t n_env, i
         for (int j = 0; j < m->njoints; ++j) {
             JointMap& jm = jmap[j];
             jm = JointMap{-1, 0, j ? m->parent[j] : 0, j ? m->idx_q[j] : 0, j ? m->idx_v[j] : 0, 0, REC_PAD, 0};
+            b->h_joint_parent.push_back(jm.parent);
             if (!j) continue;
             int found = 0;
             for (int r = 0; r < P.nrec; ++r)
@@ -650,6 +713,10 @@ int jb_describe(JbBatch* b, char* buf, int32_t len) {
         const size_t used = std::strlen(buf);
         if (used + 1 < static_cast<size_t>(len)) std::snprintf(buf + used, len - used, "; per-env flexibility parameters");
     }
+    if (b->kp.pem_on) {
+        const size_t used = std::strlen(buf);
+        if (used + 1 < static_cast<size_t>(len)) std::snprintf(buf + used, len - used, "; per-env model rows");
+    }
     for (int j = 0; j < b->kp.n_proc; ++j) {
         const size_t used = std::strlen(buf);
         if (used + 1 >= static_cast<size_t>(len)) break;
@@ -677,6 +744,7 @@ int jb_set_options(JbBatch* b, const JbOptions* o) {
 // and every group of envs that shares a warp uses one of them (a table base per block: nothing on the hot path changes).
 int jb_set_model_variants(JbBatch* b, int32_t n_variants, const JbModelDesc* models, const int32_t* variant_of_group) {
     if (!b || !models || !variant_of_group || n_variants < 1) return fail(JB_ERR_INVALID_ARGUMENT, "null argument");
+    if (b->kp.pem_on) return fail(JB_ERR_BAD_CONTROL_FLOW, "the batch has per-env model rows (jb_enable_per_env_model): set them with jb_set_model_env");
     CU(cudaSetDevice(b->device));
     const Plan& P0 = b->plan;
     const int epw = 32 / P0.L, ngroups = (b->n_env + epw - 1) / epw;
@@ -838,6 +906,149 @@ int jb_get_flexibility_env(JbBatch* b, double* out) {
     CU(cudaSetDevice(b->device));
     CU(cudaMemcpyAsync(out, b->d_flex_active, static_cast<size_t>(b->n_env) * 6 * b->kp.n_flex * sizeof(double), cudaMemcpyDeviceToHost, b->stream));
     CU(cudaStreamSynchronize(b->stream));
+    return JB_OK;
+}
+
+// Per-env model rows (Model::addBiasedToExtendedModel, model.cc:1166-1236, re-applied at every reset by Model::reset,
+// model.cc:398-416): every env runs its own copy of the double table, whose inertias and joint-placement translations
+// each start takes from the env's pending row [njoints][PEM_W].
+int jb_enable_per_env_model(JbBatch* b) {
+    if (!b) return fail(JB_ERR_INVALID_ARGUMENT, "null argument");
+    if (b->kp.pem_on) return fail(JB_ERR_INVALID_ARGUMENT, "per-env model rows are already enabled");
+    const Plan& P = b->plan;
+    const int L = P.L, nj = b->kp.njoints, n = b->n_env;
+    const size_t R = P.rdbl.size();
+    if (static_cast<long long>(n) * static_cast<long long>(R) >= PEM_MAX_ROWS)
+        return fail(JB_ERR_INVALID_ARGUMENT, "per-env model rows: n_env * rows per model (" + std::to_string(n) + " * " + std::to_string(R) +
+                                                 ") must be below 2^23, the row offsets the step kernel carries in its context word");
+    // the first (record, sub-lane) row that holds each joint, and the joints the model leaves massless
+    std::vector<int32_t> jrow(nj, -1), massless(nj, 0);
+    for (int r = 0; r < P.nrec; ++r)
+        for (int s = 0; s < L; ++s) {
+            const RecInt& ri = P.rint[static_cast<size_t>(r) * L + s];
+            if (ri.kind != REC_PAD && jrow[ri.joint] < 0) jrow[ri.joint] = r * L + s;
+        }
+    for (int j = 1; j < nj; ++j) massless[j] = jrow[j] >= 0 && P.rdbl[jrow[j]].inertia[0] == 0.0 ? 1 : 0;
+    // initial tables: each env's model values (the variant of its group, if any)
+    const int epw = 32 / L;
+    const bool variants = !b->h_variant_rows.empty();
+    std::vector<RecDbl> rows(static_cast<size_t>(n) * R);
+    std::vector<double> pend(static_cast<size_t>(n) * nj * PEM_W, 0.0), sub(nj), mass(n);
+    for (int e = 0; e < n; ++e) {
+        const RecDbl* src = variants ? &b->h_variant_rows[static_cast<size_t>(b->h_variant_of_group[e / epw]) * R] : P.rdbl.data();
+        std::copy(src, src + R, rows.begin() + static_cast<size_t>(e) * R);
+        double* x = &pend[static_cast<size_t>(e) * nj * PEM_W];
+        for (int j = 1; j < nj; ++j) {
+            if (jrow[j] < 0) continue;
+            const RecDbl& rd = src[jrow[j]];
+            for (int k = 0; k < 10; ++k) x[j * PEM_W + k] = rd.inertia[k];
+            for (int k = 0; k < 3; ++k) x[j * PEM_W + 10 + k] = rd.placement[9 + k];
+        }
+        // the total mass as build_plan sums it
+        sub[0] = 0.0;
+        for (int j = 1; j < nj; ++j) sub[j] = x[j * PEM_W];
+        for (int j = nj - 1; j > 0; --j) sub[b->h_joint_parent[j]] += sub[j];
+        mass[e] = sub[0];
+    }
+    CU(cudaSetDevice(b->device));
+    RecDbl* d_rows; int32_t *d_parent, *d_bad; double *d_sub, *d_mass;
+    int rc;
+    if ((rc = dev_alloc(b, &d_rows, rows.size())) || (rc = dev_alloc(b, &b->d_pem_pending, pend.size())) ||
+        (rc = dev_alloc(b, &b->d_pem_stage, pend.size())) || (rc = dev_alloc(b, &d_sub, static_cast<size_t>(n) * nj)) ||
+        (rc = dev_alloc(b, &d_mass, mass.size())) || (rc = dev_alloc(b, &d_bad, n)) || (rc = dev_alloc(b, &d_parent, nj)) ||
+        (rc = dev_alloc(b, &b->d_pem_massless, nj)))
+        return rc;
+    CU(cudaMemcpyAsync(d_rows, rows.data(), rows.size() * sizeof(RecDbl), cudaMemcpyHostToDevice, b->stream));
+    CU(cudaMemcpyAsync(b->d_pem_pending, pend.data(), pend.size() * sizeof(double), cudaMemcpyHostToDevice, b->stream));
+    CU(cudaMemcpyAsync(d_mass, mass.data(), mass.size() * sizeof(double), cudaMemcpyHostToDevice, b->stream));
+    CU(cudaMemcpyAsync(d_parent, b->h_joint_parent.data(), nj * sizeof(int32_t), cudaMemcpyHostToDevice, b->stream));
+    CU(cudaMemcpyAsync(b->d_pem_massless, massless.data(), nj * sizeof(int32_t), cudaMemcpyHostToDevice, b->stream));
+    CU(cudaStreamSynchronize(b->stream));   // the host vectors go away
+    b->h_pem_row = jrow;
+    b->h_pem_massless = massless;
+    KParams& kp = b->kp;
+    kp.pem_on = 1;
+    kp.rdbl = d_rows; kp.rdbl_rows = static_cast<int32_t>(R);
+    kp.pem_parent = d_parent; kp.pem_pending = b->d_pem_pending; kp.pem_rows = d_rows; kp.pem_subtree = d_sub;
+    kp.pem_mass = d_mass; kp.pem_bad = d_bad;
+    return JB_OK;
+}
+
+// Masked pending rows, one thread per env.  A row with a value that is not finite, or a mass that is not positive (zero
+// is kept where the model's body is massless), is not written and flags its env (its next start refuses it); a valid
+// row clears the flag.  Joint 0 (the universe) is neither checked nor written.
+__global__ void set_model_rows_kernel(double* __restrict__ pending, int32_t* __restrict__ bad_flag, const uint8_t* __restrict__ mask,
+                                      const double* __restrict__ rows, const int32_t* __restrict__ massless, int n_env, int nj) {
+    const int e = blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= n_env || (mask && !mask[e])) return;
+    const size_t o = static_cast<size_t>(e) * nj * PEM_W;
+    bool bad = false;
+    for (int j = 1; j < nj; ++j) {
+        const double* x = rows + o + j * PEM_W;
+        for (int k = 0; k < PEM_W; ++k) bad = bad || !(fabs(x[k]) <= 1.7976931348623157e308);
+        bad = bad || !(x[0] > 0.0 || (x[0] == 0.0 && massless[j]));
+    }
+    bad_flag[e] = bad ? 1 : 0;
+    if (bad) return;
+    for (int k = PEM_W; k < nj * PEM_W; ++k) pending[o + k] = rows[o + k];
+}
+
+static int launch_model_rows(JbBatch* b, const uint8_t* mask_dev, const double* rows) {
+    JB_LAUNCH(set_model_rows_kernel, static_cast<unsigned>((b->n_env + 127) / 128), 128, 0, b->stream, b->d_pem_pending,
+              b->kp.pem_bad, mask_dev, rows, b->d_pem_massless, b->n_env, b->kp.njoints);
+    CU(cudaGetLastError());
+    ++b->launches;
+    return JB_OK;
+}
+
+int jb_set_model_env(JbBatch* b, const uint8_t* mask, const double* rows) {
+    if (!b || !rows) return fail(JB_ERR_INVALID_ARGUMENT, "null argument");
+    if (!b->kp.pem_on) return fail(JB_ERR_BAD_CONTROL_FLOW, "per-env model rows are not enabled (jb_enable_per_env_model)");
+    CU(cudaSetDevice(b->device));
+    const int nj = b->kp.njoints;
+    for (int e = 0; e < b->n_env; ++e) {
+        if (mask && !mask[e]) continue;
+        for (int j = 1; j < nj; ++j) {
+            const double* x = rows + (static_cast<size_t>(e) * nj + j) * PEM_W;
+            for (int k = 0; k < PEM_W; ++k)
+                if (!std::isfinite(x[k])) return fail(JB_ERR_INVALID_ARGUMENT, "model rows must be finite (env " + std::to_string(e) + ", joint " + std::to_string(j) + ").");
+            if (!(x[0] > 0.0 || (x[0] == 0.0 && b->h_pem_massless[j])))
+                return fail(JB_ERR_INVALID_ARGUMENT, "the mass of a body must be positive (env " + std::to_string(e) + ", joint " + std::to_string(j) + ").");
+        }
+    }
+    CU(cudaMemcpyAsync(b->d_pem_stage, rows, static_cast<size_t>(b->n_env) * nj * PEM_W * sizeof(double), cudaMemcpyHostToDevice, b->stream));
+    if (mask) CU(cudaMemcpyAsync(b->d_mask, mask, b->n_env, cudaMemcpyHostToDevice, b->stream));
+    int rc = launch_model_rows(b, mask ? b->d_mask : nullptr, b->d_pem_stage);
+    if (rc) return rc;
+    CU(cudaStreamSynchronize(b->stream));
+    return JB_OK;
+}
+
+int jb_set_model_env_device(JbBatch* b, const uint8_t* mask_dev, const double* rows_dev) {
+    if (!b || !rows_dev) return fail(JB_ERR_INVALID_ARGUMENT, "null argument");
+    if (!b->kp.pem_on) return fail(JB_ERR_BAD_CONTROL_FLOW, "per-env model rows are not enabled (jb_enable_per_env_model)");
+    CU(cudaSetDevice(b->device));
+    return launch_model_rows(b, mask_dev, rows_dev);
+}
+
+int jb_get_model_env(JbBatch* b, double* out) {
+    if (!b || !out) return fail(JB_ERR_INVALID_ARGUMENT, "null argument");
+    if (!b->kp.pem_on) return fail(JB_ERR_BAD_CONTROL_FLOW, "per-env model rows are not enabled (jb_enable_per_env_model)");
+    CU(cudaSetDevice(b->device));
+    const size_t R = static_cast<size_t>(b->kp.rdbl_rows);
+    const int nj = b->kp.njoints;
+    std::vector<RecDbl> rows(static_cast<size_t>(b->n_env) * R);
+    CU(cudaMemcpyAsync(rows.data(), b->kp.pem_rows, rows.size() * sizeof(RecDbl), cudaMemcpyDeviceToHost, b->stream));
+    CU(cudaStreamSynchronize(b->stream));
+    std::fill(out, out + static_cast<size_t>(b->n_env) * nj * PEM_W, 0.0);
+    for (int e = 0; e < b->n_env; ++e)
+        for (int j = 1; j < nj; ++j) {
+            if (b->h_pem_row[j] < 0) continue;
+            const RecDbl& rd = rows[static_cast<size_t>(e) * R + b->h_pem_row[j]];
+            double* x = out + (static_cast<size_t>(e) * nj + j) * PEM_W;
+            for (int k = 0; k < 10; ++k) x[k] = rd.inertia[k];
+            for (int k = 0; k < 3; ++k) x[10 + k] = rd.placement[9 + k];
+        }
     return JB_OK;
 }
 

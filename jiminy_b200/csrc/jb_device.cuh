@@ -194,6 +194,17 @@ struct KParams {
     const double* flex_pending;    // [n_env][n_flex][6] rows written by the setters
     double* flex_active;           // [n_env][n_flex][6] rows latched at the env's last start
     int32_t* flex_bad;             // [n_env] 1: the last device row was rejected, the env's next start refuses it
+    // per-env model rows (jb_enable_per_env_model): `rdbl` is one table of rdbl_rows rows per env, read by the
+    // env_step_kernel_model instances through Ctx::flags; before every start latch_model_rows_kernel expands the env's
+    // pending row [njoints][PEM_W]
+    // (mass, lever xyz, inertia about the centre of mass xx xy yy xz yz zz, joint-placement translation xyz) into it
+    int32_t pem_on;
+    const int32_t* pem_parent;     // [njoints] parent joint (parents precede children)
+    const double* pem_pending;     // [n_env][njoints][PEM_W] rows written by the setters
+    RecDbl* pem_rows;              // [n_env][rdbl_rows] the tables the envs run with (== rdbl)
+    double* pem_subtree;           // [n_env][njoints] subtree masses (scratch of the latch)
+    double* pem_mass;              // [n_env] total mass of the env's model
+    int32_t* pem_bad;              // [n_env] 1: the last device row was rejected, the env's next start refuses it
 };
 
 // Launch parameters live in constant memory (uniform constant-bank operands in every device
@@ -228,6 +239,10 @@ __device__ unsigned long long jb_prof[16];
 // variants) -- a shift and an add where the tables are read, no register and no memory access of its own
 constexpr int CTX_ROW_SHIFT = 8;
 #define JB_RDBL (KP->rdbl + (c.flags >> CTX_ROW_SHIFT))
+// per-env model rows: doubles of one joint's pending row, and the bound on the row offsets the flags carry
+// (n_env * rdbl_rows)
+constexpr int PEM_W = 13;
+constexpr long long PEM_MAX_ROWS = 1LL << (31 - CTX_ROW_SHIFT);
 
 // ------------------------------------------------------------------------------------------
 // small fixed-size algebra in registers
@@ -2812,6 +2827,8 @@ __device__ constexpr int X1_H = R1_FU;                                    // 6
 __device__ constexpr int X1_FE[6] = {R1_DINV, R1_U, R1_QS, R1_QS + 1, R1_VS, R1_SV};
 __device__ constexpr int XF_H = RF_QS, XF_FE = RF_VS;                     // 6 + 6
 
+// MODEL: the batch has per-env model rows (env_step_kernel_model): the env's own total mass
+template <bool MODEL = false>
 __device__ __noinline__ void extra_terms(const Ctx c) {
     const int L = KP->L;
     const JbOptions& opt = KP->opt;
@@ -3012,7 +3029,7 @@ __device__ __noinline__ void extra_terms(const Ctx c) {
             double* o = KP->extra_com + col * KP->njoints * 3;
             o[0] = com0.x; o[1] = com0.y; o[2] = com0.z;
             double* w = KP->extra_vcom + col * KP->njoints * 3;
-            const double mtot = KP->block_mass != nullptr ? KP->block_mass[blockIdx.x] : KP->total_mass;
+            const double mtot = MODEL ? KP->pem_mass[col] : (KP->block_mass != nullptr ? KP->block_mass[blockIdx.x] : KP->total_mass);
             w[0] = h0.l.x / mtot; w[1] = h0.l.y / mtot; w[2] = h0.l.z / mtot;
             double* y = KP->extra_ycrb + col * KP->njoints * 10;
 #pragma unroll

@@ -430,7 +430,10 @@ __device__ __noinline__ void store_dynamics(const Ctx c) {
 // scheduler iteration (impulse breakpoints, FSAL repair on a change), process forces before every evaluation.
 // FLEX (full body only): the batch has per-env flexibility parameters (env_step_kernel_flex): each start latches the
 // env's pending row, and the sweeps read the active rows.
-template <bool FAST, bool EXT = false, bool FLEX = false>
+// MODEL: the batch has per-env model rows (env_step_kernel_model): every lane reads its env's own table (the row offset in
+// Ctx::flags), a start refuses an env whose last device row was rejected, and the centroidal terms divide by the env's
+// total mass.
+template <bool FAST, bool EXT = false, bool FLEX = false, bool MODEL = false>
 __device__ __forceinline__ void env_step_body(const LaunchArgs& la, const bool only_flagged) {
     static_assert(FAST || !EXT, "external forces on the full body need no instance of their own");
     Ctx c;
@@ -441,7 +444,8 @@ __device__ __forceinline__ void env_step_body(const LaunchArgs& la, const bool o
     const int env_raw = blockIdx.x * epw + c.lane / L;
     c.valid = env_raw < KP->n_env;
     c.env = c.valid ? env_raw : (KP->n_env - 1);
-    c.flags = KP->n_variants > 1 ? (KP->variant_of_block[blockIdx.x] * KP->rdbl_rows) << CTX_ROW_SHIFT : 0;
+    if constexpr (MODEL) c.flags = (c.env * KP->rdbl_rows) << CTX_ROW_SHIFT;
+    else c.flags = KP->n_variants > 1 ? (KP->variant_of_block[blockIdx.x] * KP->rdbl_rows) << CTX_ROW_SHIFT : 0;
     c.gmask = (L == 32) ? 0xffffffffu : (((1u << L) - 1u) << (c.lane - c.sub));
     const size_t N = KP->n_pad, col = c.env;
     const int mode = la.mode;
@@ -450,6 +454,12 @@ __device__ __forceinline__ void env_step_body(const LaunchArgs& la, const bool o
     const bool masked_out = (mode == MODE_START) && la.mask != nullptr && la.mask[c.env] == 0;
     if (masked_out) return;   // whole env (all its lanes) leaves: group masks keep the others safe
     if constexpr (!FAST) {
+        // per-env model rows: refused if the last device row for this env was.  Otherwise the launch before this one
+        // (latch_model_rows_kernel) has made the pending row the model the episode runs with, grounding included.
+        if (MODEL && mode == MODE_START && KP->pem_bad[c.env] != 0) {
+            if (c.valid && c.sub == 0) KP->status[c.env] = JB_ENV_NOT_STARTED | JB_ENV_BAD_START;
+            return;
+        }
         if (mode == MODE_START && la.ground) place_on_ground(c);
         // jb_start_device: the input checks jb_start runs on the host (Engine::start, engine.cc:1007-1037), per env.  An env
         // whose row fails them is not started and writes nothing but its status word.
@@ -782,7 +792,7 @@ __device__ __forceinline__ void env_step_body(const LaunchArgs& la, const bool o
             if (c.sub == 0) CST(CS_SOLVE_FAILED) = SMF(c, KP->rec_off[1] + R1_BFAIL);
         }
     }
-    if (KP->extra_energy != nullptr && !(status & (JB_ENV_NAN | JB_ENV_NOT_STARTED))) extra_terms(c);
+    if (KP->extra_energy != nullptr && !(status & (JB_ENV_NAN | JB_ENV_NOT_STARTED))) extra_terms<MODEL>(c);
     store_outputs(c);
 #ifndef JB_HOST_EMUL
     // multi-GPU: publish the sensor rows into every rank's gathered buffer (stores over NVLink / NVSwitch).  The rows
@@ -842,28 +852,28 @@ JB_DI unsigned int jb_smid() {
 
 // The full body: every mode, every stepper, the constraint path.  Out of line, so that the hot-path kernel carries one
 // call to it instead of a second copy of the code.
-template <bool FLEX = false>
+template <bool FLEX = false, bool MODEL = false>
 __device__ __noinline__ void env_step_full(const LaunchArgs la, const bool only_flagged) {
     // constraint workspace of this block: one row per block of the launch.  (A pool of per-SM slots taken with an atomic
     // spin by lane 0 kept the workspace L2-resident, but left the warp's env groups running one after the other in the
     // constraint solvers -- several times slower on ANYmal with constraint contacts.)
     if (threadIdx.x == 0) jb_cw_slot = static_cast<int>(blockIdx.x);
     __syncwarp();
-    env_step_body<false, false, FLEX>(la, only_flagged);
+    env_step_body<false, false, FLEX, MODEL>(la, only_flagged);
 }
 
 // One launch = one Engine::step (or start / single evaluation) of every env.  FAST: the hot-path body first; the envs it
 // handed over (a joint left its bounds now, or constraints still enabled from an earlier step) go through the full
 // body in the same launch, so a step is always exactly one kernel.  EXT: the hot-path body is the force-carrying one.
-template <bool FAST, bool EXT, bool FLEX = false>
+template <bool FAST, bool EXT, bool FLEX = false, bool MODEL = false>
 __device__ __forceinline__ void env_step_launch(const LaunchArgs& la) {
     JB_PROF_T(t_kernel);
     if constexpr (FAST) {
-        env_step_body<true, EXT>(la, false);
+        env_step_body<true, EXT, false, MODEL>(la, false);
         __syncwarp();   // needs_full is written by sub-lane 0 of each env
         const int flag = KP->needs_full[blockIdx.x * (32 / KP->L) + (threadIdx.x & 31) / KP->L];
-        if (__any_sync(0xffffffffu, flag != 0)) env_step_full(la, true);
-    } else env_step_full<FLEX>(la, false);
+        if (__any_sync(0xffffffffu, flag != 0)) env_step_full<false, MODEL>(la, true);
+    } else env_step_full<FLEX, MODEL>(la, false);
     JB_PROF_ADD(6, t_kernel);                              // the whole kernel
     JB_PROF_COUNT(7, 1);                                   // warps
 #ifndef JB_HOST_EMUL
@@ -891,6 +901,12 @@ __global__ void __launch_bounds__(32) env_step_kernel_ext(const LaunchArgs la) {
 // Batches with per-env flexibility parameters (jb_enable_per_env_flexibility): every launch runs the full body with the
 // sweep instances that read the env's active rows (SigDynamicFlex), so the kernels above are not touched.
 __global__ void __launch_bounds__(32) env_step_kernel_flex(const LaunchArgs la) { env_step_launch<false, false, true>(la); }
+// Batches with per-env model rows (jb_enable_per_env_model): the four kernels above, with every env reading its own
+// table and its own total mass (MODEL).  The kernels above are not touched.
+__global__ void __launch_bounds__(32) env_step_kernel_model_fast(const LaunchArgs la) { env_step_launch<true, false, false, true>(la); }
+__global__ void __launch_bounds__(32) env_step_kernel_model_ext(const LaunchArgs la) { env_step_launch<true, true, false, true>(la); }
+__global__ void __launch_bounds__(32) env_step_kernel_model(const LaunchArgs la) { env_step_launch<false, false, false, true>(la); }
+__global__ void __launch_bounds__(32) env_step_kernel_model_flex(const LaunchArgs la) { env_step_launch<false, false, true, true>(la); }
 
 // ---- observation exchange over peer memory: the consumer's wait (one thread)
 #ifndef JB_HOST_EMUL

@@ -102,12 +102,16 @@ def configure_pd_blocks(env, kp, kd, joint_position_margin: float, joint_velocit
 
 class BatchedJiminyEnv:
     def __init__(self, scenario: scenarios.Scenario, device: int = 0, height_threshold_ratio: float = 0.5,
-                 simulation_duration_max: float = 20.0, api_: Optional[core.Api] = None, std_ratio: Optional[dict] = None):
+                 simulation_duration_max: float = 20.0, api_: Optional[core.Api] = None, std_ratio: Optional[dict] = None,
+                 model_bias_std: Optional[dict] = None):
         """`std_ratio`: the reference walker env's randomisation ratios.  None or {}: none; "disturbance": r, the walker
         disturbance forces (`jiminy_b200.disturbance`); "sensors": r, noise, bias, delay and jitter of every sensor and a
         new seed of its generators (`jiminy_b200.sensor_randomisation`); "model": r, stiffness and damping of every
-        flexibility joint (`jiminy_b200.model_randomisation`; NotImplementedError on a robot without one).  All are re-drawn for every
-        env that (re)starts."""
+        flexibility joint (`jiminy_b200.model_randomisation`; NotImplementedError on a robot without one).
+        `model_bias_std`: the body biases of the robot options `massBodiesBiasStd`, `centerOfMassPositionBodiesBiasStd`,
+        `inertiaBodiesBiasStd`, `relativePositionBodiesBiasStd` (standard deviations; None, {} or zeros: none), drawn per
+        env around the nominal model (`model_randomisation.ModelBiasRandomisation`).  All are re-drawn for every env that
+        (re)starts."""
         self.sc = scenario
         self.robot: RobotTable = scenario.robot
         self.n_env, self.step_dt = scenario.n_env, scenario.step_dt
@@ -141,6 +145,11 @@ class BatchedJiminyEnv:
             self.model_randomisation.register(self.engine)
             self._model_rng = np.random.default_rng([scenario.seed, 0xF1E8])
             self.model_rows: Optional[np.ndarray] = None     # the flexibility rows every env runs with [n_env, n_flex, 6]
+        self.model_bias = model_randomisation.from_model_bias_std(self.robot, model_bias_std)
+        if self.model_bias is not None:
+            self.model_bias.register(self.engine)
+            self._model_bias_rng = np.random.default_rng([scenario.seed, 0xB1A5])
+            self.model_bias_rows: Optional[np.ndarray] = None     # the body rows every env runs with [n_env, njoints, 13]
         self._started = False
 
     # ------------------------------------------------------------------ helpers
@@ -185,6 +194,19 @@ class BatchedJiminyEnv:
             self.model_rows = draw
             self.model_randomisation.apply_host(self.engine, draw, mask)
 
+    def _redraw_model_bias(self, mask: Optional[np.ndarray]) -> None:
+        """New body biases for the envs about to (re)start (Model::reset re-draws them at every reset, model.cc:398-416)."""
+        if self.model_bias is not None:
+            if mask is None or self.model_bias_rows is None:
+                draw = self.model_bias.draw_numpy(self._model_bias_rng, self.n_env)
+            else:
+                # only the restarting envs draw: the transformation costs host time per row
+                sel = np.flatnonzero(np.asarray(mask))
+                draw = self.model_bias_rows.copy()
+                draw[sel] = self.model_bias.draw_numpy(self._model_bias_rng, len(sel))
+            self.model_bias_rows = draw
+            self.model_bias.apply_host(self.engine, draw, mask)
+
     # ------------------------------------------------------------------ gym API
     def reset(self, mask: Optional[np.ndarray] = None) -> Tuple[Dict[str, Any], Dict[str, Any]]:
         if mask is None or not self._started:
@@ -193,6 +215,7 @@ class BatchedJiminyEnv:
             self._redraw_disturbance(None)
             self._redraw_sensors(None)
             self._redraw_model(None)
+            self._redraw_model_bias(None)
             self.engine.start(q0, v0)
             self.num_steps[:] = 0
             self._started = True
@@ -201,6 +224,7 @@ class BatchedJiminyEnv:
             self._redraw_disturbance(mask)
             self._redraw_sensors(mask)
             self._redraw_model(mask)
+            self._redraw_model_bias(mask)
             self.engine.start(q0, v0, mask=mask)
             self.num_steps[mask.astype(bool)] = 0
         return self._observation(), {}
@@ -270,6 +294,7 @@ class PDControlBatchedEnv(BatchedJiminyEnv):
             self._redraw_disturbance(None)
             self._redraw_sensors(None)
             self._redraw_model(None)
+            self._redraw_model_bias(None)
             self.engine.start(q0, v0)
             self.num_steps[:] = 0
             self._started = True

@@ -1084,46 +1084,125 @@ def _exp3(w: np.ndarray) -> np.ndarray:
     return np.eye(3) + math.sin(th) / th * K + (1.0 - math.cos(th)) / (th * th) * (K @ K)
 
 
+BIAS_EPS = 2.220446049250313e-16
+
+
+def bias_normals(mass_std: float = 0.0, com_std: float = 0.0, inertia_std: float = 0.0,
+                 relative_position_std: float = 0.0) -> int:
+    """Standard normals one mechanical joint of `bias_bodies` consumes: centre of mass 3, mass 1, inertia axes 3 and
+    moments 3, translation 3, for the standard deviations above machine epsilon."""
+    return (3 * (com_std > BIAS_EPS) + (mass_std > BIAS_EPS) + 6 * (inertia_std > BIAS_EPS) +
+            3 * (relative_position_std > BIAS_EPS))
+
+
+def bias_bodies(inertia: np.ndarray, translation: np.ndarray, z: np.ndarray, eig, *, mass_std: float = 0.0,
+                com_std: float = 0.0, inertia_std: float = 0.0, relative_position_std: float = 0.0):
+    """Mechanical joints of `Model::addBiasedToExtendedModel` (core/src/robot/model.cc:1166-1236), batched over leading
+    axes: returns new arrays of the joints' inertias [..., 10] (mass, lever, inertia about the centre of mass xx xy yy xz
+    yz zz) and joint-placement translations [..., 3].  `z` [..., bias_normals]: each joint's single-precision standard
+    normals, in the reference's order; `eig`: (moments [..., 3], axes [..., 3, 3]) of `np.linalg.eigh` of each joint's
+    rotational inertia (broadcast against the leading axes).
+    - the lever is scaled component-wise by N(1, com_std);
+    - the mass by N(1, mass_std), never below min(mass, 1 g);
+    - the principal axes are turned by the rotation vector N(0, inertia_std) (pinocchio::exp3) and the principal moments
+      scaled by N(1, inertia_std);
+    - the translation is scaled component-wise by N(1, relative_position_std).
+    Each normal is formed in single precision (mean + std z), like the reference's draws.  Every operation is the one a
+    single joint would take (elementwise ops, `dot` for the norm of the rotation vector, `math.sin` / `math.cos`,
+    stacked `matmul`), so that a batch gives the bits of its joints drawn one at a time."""
+    lead = np.broadcast_shapes(np.shape(inertia)[:-1], np.shape(z)[:-1])
+    inertia = np.array(np.broadcast_to(inertia, lead + (10,)), dtype=np.float64, copy=True)
+    translation = np.array(np.broadcast_to(translation, lead + (3,)), dtype=np.float64, copy=True)
+    k = 0
+
+    def normal(n, mean, std):
+        nonlocal k
+        x = (np.float32(mean) + np.float32(std) * z[..., k:k + n]).astype(np.float64)
+        k += n
+        return x
+    if com_std > BIAS_EPS:
+        inertia[..., 1:4] *= normal(3, 1.0, com_std)
+    if mass_std > BIAS_EPS:
+        m = inertia[..., 0]
+        inertia[..., 0] = np.maximum(m * normal(1, 1.0, mass_std)[..., 0], np.minimum(m, 1.0e-3))
+    if inertia_std > BIAS_EPS:
+        moments, axes = eig
+        w = normal(3, 0.0, inertia_std)
+        flat = w.reshape(-1, 3)
+        th = np.sqrt(np.array([r.dot(r) for r in flat])).reshape(lead)     # np.linalg.norm of each rotation vector
+        sin = np.array([math.sin(t) for t in th.ravel()]).reshape(lead)
+        cos = np.array([math.cos(t) for t in th.ravel()]).reshape(lead)
+        zero = np.zeros(lead)
+        K = np.stack([zero, -w[..., 2], w[..., 1], w[..., 2], zero, -w[..., 0], -w[..., 1], w[..., 0], zero], -1).reshape(lead + (3, 3))
+        small = (th < 1e-12)[..., None, None]
+        with np.errstate(divide="ignore", invalid="ignore"):
+            big = np.eye(3) + (sin / th)[..., None, None] * K + ((1.0 - cos) / (th * th))[..., None, None] * (K @ K)
+        R = np.where(small, np.eye(3) + K, big)
+        ax = np.broadcast_to(axes, lead + (3, 3)) @ R
+        mo = moments * normal(3, 1.0, inertia_std)
+        D = np.zeros(lead + (3, 3))
+        for a in range(3):
+            D[..., a, a] = mo[..., a]
+        I = ax @ D @ np.swapaxes(ax, -1, -2)
+        inertia[..., 4:10] = np.stack([I[..., 0, 0], I[..., 0, 1], I[..., 1, 1], I[..., 0, 2], I[..., 1, 2], I[..., 2, 2]], -1)
+    if relative_position_std > BIAS_EPS:
+        translation *= normal(3, 1.0, relative_position_std)
+    return inertia, translation
+
+
+def inertia_eig(inertia: np.ndarray):
+    """`np.linalg.eigh` of each rotational inertia of inertia rows [J, 10], one joint at a time: (moments [J, 3],
+    axes [J, 3, 3])."""
+    out = []
+    for row in np.asarray(inertia, dtype=np.float64).reshape(-1, 10):
+        xx, xy, yy, xz, yz, zz = row[4:10]
+        out.append(np.linalg.eigh(np.array([[xx, xy, xz], [xy, yy, yz], [xz, yz, zz]])))
+    return np.array([m for m, _ in out]).reshape(-1, 3), np.array([a for _, a in out]).reshape(-1, 3, 3)
+
+
+def bias_joints(robot: RobotTable) -> List[int]:
+    """The joints `addBiasedToExtendedModel` biases: the mechanical joints (`mechanicalJointNames_`), in the reference's
+    order -- neither the root free-flyer nor the flexibility joints inserted into the extended model."""
+    return [j for j in range(1, robot.njoints) if int(robot.joint_type[j]) != JB_JOINT_FREEFLYER and
+            robot.joint_names[j] not in robot.flexibility_joint_names]
+
+
+def body_rows(robot: RobotTable) -> np.ndarray:
+    """Per joint [njoints, 13]: mass, lever xyz, inertia about the centre of mass (xx xy yy xz yz zz), joint-placement
+    translation xyz -- the layout of `BatchedEngine.set_model_env`.  Row 0 (the universe) is zero."""
+    rows = np.concatenate([np.asarray(robot.inertia, dtype=np.float64), np.asarray(robot.placement, dtype=np.float64)[:, 9:12]], 1)
+    rows[0] = 0.0
+    return rows
+
+
+def with_body_rows(robot: RobotTable, rows: np.ndarray) -> RobotTable:
+    """`robot` with the inertias and joint-placement translations of `rows` [njoints, 13] (`body_rows`' layout, row 0
+    ignored); everything else is shared with `robot`."""
+    import copy
+    out = copy.copy(robot)
+    out.inertia = np.array(robot.inertia, dtype=np.float64, copy=True)
+    out.placement = np.array(robot.placement, dtype=np.float64, copy=True)
+    out.inertia[1:] = rows[1:, :10]
+    out.placement[1:, 9:12] = rows[1:, 10:13]
+    return out
+
+
 def biased_robot(robot: RobotTable, rng: np.random.Generator, *, mass_std: float = 0.0, com_std: float = 0.0,
                  inertia_std: float = 0.0, relative_position_std: float = 0.0) -> RobotTable:
     """One draw of `Model::addBiasedToExtendedModel` (core/src/robot/model.cc:1166-1236) with the model options
     `massBodiesBiasStd`, `centerOfMassPositionBodiesBiasStd`, `inertiaBodiesBiasStd`, `relativePositionBodiesBiasStd`:
-    for every mechanical joint (not the root free-flyer), in the reference's order, the centre of mass is scaled
-    component-wise by N(1, std), the mass by N(1, std) (never below min(mass, 1 g)), the principal moments of inertia by
-    N(1, std) after the principal axes have been turned by a random rotation vector N(0, std), and the translation of the
-    joint placement by N(1, std) (rotation untouched).  Draws are single precision like the reference's; the stream is
-    numpy's, not the engine's PCG32 (and Eigen's eigenvector signs are not reproduced): equal in distribution, not draw by
-    draw.  Returns a new table; everything but `inertia` and `placement` is shared with `robot`."""
+    `bias_bodies` on every mechanical joint (`bias_joints`), in the reference's order.  Draws are single precision like
+    the reference's; the stream is numpy's, not the engine's PCG32 (and Eigen's eigenvector signs are not reproduced):
+    equal in distribution, not draw by draw.  Order of the reference (Model / Robot::initializeExtendedModel):
+    flexibilities, then the biases, then the backlash joints -- call `add_backlash_joints` on the biased table, not
+    before.  Returns a new table; everything but `inertia` and `placement` is shared with `robot`."""
     import copy
-    EPS = 2.220446049250313e-16
     out = copy.copy(robot)
     out.inertia = np.array(robot.inertia, dtype=np.float64, copy=True)
     out.placement = np.array(robot.placement, dtype=np.float64, copy=True)
-
-    def normal(n, mean, std):
-        return (np.float32(mean) + np.float32(std) * rng.standard_normal(n, dtype=np.float32)).astype(np.float64)
-    for j in range(1, robot.njoints):
-        if int(robot.joint_type[j]) == JB_JOINT_FREEFLYER:
-            continue
-        # `mechanicalJointNames_` only: the joints of the theoretical model, not the flexibility joints inserted into the
-        # extended one.  Order of the reference (Model / Robot::initializeExtendedModel): flexibilities, then the biases,
-        # then the backlash joints -- call `add_backlash_joints` on the biased table, not before.
-        if robot.joint_names[j] in robot.flexibility_joint_names:
-            continue
-        if com_std > EPS:
-            out.inertia[j, 1:4] *= normal(3, 1.0, com_std)
-        if mass_std > EPS:
-            m = out.inertia[j, 0]
-            out.inertia[j, 0] = max(m * float(normal(1, 1.0, mass_std)[0]), min(m, 1.0e-3))
-        if inertia_std > EPS:
-            xx, xy, yy, xz, yz, zz = out.inertia[j, 4:10]
-            I = np.array([[xx, xy, xz], [xy, yy, yz], [xz, yz, zz]])
-            moments, axes = np.linalg.eigh(I)
-            axes = axes @ _exp3(normal(3, 0.0, inertia_std))
-            moments = moments * normal(3, 1.0, inertia_std)
-            I = axes @ np.diag(moments) @ axes.T
-            out.inertia[j, 4:10] = [I[0, 0], I[0, 1], I[1, 1], I[0, 2], I[1, 2], I[2, 2]]
-        if relative_position_std > EPS:
-            out.placement[j, 9:12] *= normal(3, 1.0, relative_position_std)
+    stds = dict(mass_std=mass_std, com_std=com_std, inertia_std=inertia_std, relative_position_std=relative_position_std)
+    joints = bias_joints(robot)
+    z = rng.standard_normal((len(joints), bias_normals(**stds)), dtype=np.float32)
+    out.inertia[joints], out.placement[joints, 9:12] = bias_bodies(out.inertia[joints], out.placement[joints, 9:12], z,
+                                                                    inertia_eig(out.inertia[joints]), **stds)
     return out
-

@@ -41,6 +41,14 @@ re-drawn the same way (`jiminy_b200.model_randomisation`) and written by `jb_set
 masked restart, which latches them.  `env.model_rows` holds the rows every env currently runs with.  The sampler never
 draws a row the setter would reject (the ratio is checked against the nominal values at construction).
 
+Model biases.  With `model_bias_std` (the standard deviations of `massBodiesBiasStd`, `centerOfMassPositionBodiesBiasStd`,
+`inertiaBodiesBiasStd`, `relativePositionBodiesBiasStd`) the masses, centres of mass, inertias and joint-placement
+translations of the envs in the done mask are re-drawn around the nominal model with the env's torch generator
+(`model_randomisation.ModelBiasRandomisation`) and written by `jb_set_model_env_device` before the masked restart, which
+latches them.  `env.model_bias_rows` holds the rows every env currently runs with.  The restart bank, like the host envs'
+restarts, is grounded on the nominal model; only `reset_states="sample"` grounds each env on its own biased model, inside
+the start kernel.
+
 Streams.  All work runs on the batch's own stream (`torch.cuda.ExternalStream(engine.stream())`).  On entry it waits
 for the caller's current stream; on exit the caller's current stream waits for it.  With the CPU emulation of the
 library (`api_` given), device memory is host memory: the env then runs on `torch_device="cpu"`, without streams.
@@ -131,6 +139,11 @@ class DeviceBatchedEnv(envs.BatchedJiminyEnv):
             self._model_gen.manual_seed(int(np.random.default_rng([self.sc.seed, 0xF1E8]).integers(0, 2 ** 31 - 1)))
             with self._on_batch_stream():
                 self.model_rows = self.model_randomisation.draw_torch(self._model_gen, n, dev)
+        if self.model_bias is not None:
+            self._model_bias_gen = torch.Generator(device=dev)
+            self._model_bias_gen.manual_seed(int(np.random.default_rng([self.sc.seed, 0xB1A5]).integers(0, 2 ** 31 - 1)))
+            with self._on_batch_stream():
+                self.model_bias_rows = self.model_bias.draw_torch(self._model_bias_gen, n, dev)
         self.num_steps = torch.zeros(n, dtype=torch.int64, device=dev)
         # zero-copy views of the batch's device buffers
         ptr = eng.device_state_ptrs()
@@ -238,6 +251,15 @@ class DeviceBatchedEnv(envs.BatchedJiminyEnv):
         self.model_rows.copy_(new if done is None else torch.where(done.view(-1, 1, 1), new, self.model_rows))
         self.model_randomisation.apply_device(self.engine, self.model_rows, None if done is None else self._mask.data_ptr())
 
+    def _redraw_model_bias(self, done: Optional[torch.Tensor]) -> None:
+        """New body biases for the envs of `done` (None: all), drawn on the device and written by the device setter with
+        the mask in `self._mask`; `model_bias_rows` keeps what every env runs with."""
+        if self.model_bias is None:
+            return
+        new = self.model_bias.draw_torch(self._model_bias_gen, self.n_env, self.torch_device)
+        self.model_bias_rows.copy_(new if done is None else torch.where(done.view(-1, 1, 1), new, self.model_bias_rows))
+        self.model_bias.apply_device(self.engine, self.model_bias_rows, None if done is None else self._mask.data_ptr())
+
     def _restart(self, done: torch.Tensor) -> Optional[torch.Tensor]:
         """Masked restart of the envs in `done` from bank rows drawn on the device; returns the rows (-1: not restarted).
         With `reset_states="sample"`: from fresh draws put on the ground in the start kernel; returns None."""
@@ -255,6 +277,7 @@ class DeviceBatchedEnv(envs.BatchedJiminyEnv):
         self._redraw_disturbance(done)
         self._redraw_sensors(done)
         self._redraw_model(done)
+        self._redraw_model_bias(done)
         self.engine.start_device(self._q_start.data_ptr(), self._v_start.data_ptr(), self._mask.data_ptr(),
                                  on_ground=self._sample_restarts)
         self.num_steps.masked_fill_(done, 0)
@@ -272,6 +295,7 @@ class DeviceBatchedEnv(envs.BatchedJiminyEnv):
                 self._redraw_disturbance(None)
                 self._redraw_sensors(None)
                 self._redraw_model(None)
+                self._redraw_model_bias(None)
                 self.engine.start(self.sc.q0, self.sc.v0)
                 self.num_steps.zero_()
                 self._started = True

@@ -29,13 +29,18 @@ and jitter of every sensor and fresh generator seeds, re-drawn at every restart)
 turns the walker model randomisation on the same way (`std_ratio={"model": R}`: per-env stiffness and damping of every
 flexibility joint, re-drawn at every restart; r <= 2 on that robot).
 
+`--model-bias S` sets the four body-bias standard deviations of the robot options (`massBodiesBiasStd`,
+`centerOfMassPositionBodiesBiasStd`, `inertiaBodiesBiasStd`, `relativePositionBodiesBiasStd`) to S (`model_bias_std`:
+per-env masses, centres of mass, inertias and joint placements, re-drawn at every restart) and runs each loop with them
+off and on, alternating in one process, `max(--alternate, 1)` rounds; randomisation options given with it are on in both.
+
 `--restart sample` times the device loop with its restarts from fresh draws of the initial-state distribution put on the
 ground in the start kernel (`reset_states="sample"`) against the default restart bank, alternating in one process,
 `max(--alternate, 1)` rounds; randomisation options given with it are on in both.
 
     python tools/bench_pipeline.py [--robot atlas|anymal|anymal_flexible] [--loop host|device] [--alternate R]
                                    [--n-env 4096] [--steps 10] [--warmup 3] [--duration-max 0.4] [--disturbance R]
-                                   [--sensors R] [--model R] [--restart bank|sample]
+                                   [--sensors R] [--model R] [--model-bias S] [--restart bank|sample]
 """
 import argparse
 import json
@@ -55,10 +60,13 @@ KEYS = [("states", "pd_controller"), ("measurements", "EncoderSensor"), ("featur
 
 
 def make_env(n_env: int, api_=None, robot: str = "atlas", loop: str = "host", duration_max: float = 20.0,
-             disturbance: float = 0.0, sensors: float = 0.0, model: float = 0.0, restart: str = "bank"):
+             disturbance: float = 0.0, sensors: float = 0.0, model: float = 0.0, restart: str = "bank",
+             model_bias: float = 0.0):
     from jiminy_b200 import envs, scenarios
+    from jiminy_b200.model_randomisation import BIAS_OPTIONS
     ratio = {k: r for k, r in (("disturbance", disturbance), ("sensors", sensors), ("model", model)) if r > 0}
-    kw = dict(simulation_duration_max=duration_max, api_=api_, std_ratio=ratio or None)
+    kw = dict(simulation_duration_max=duration_max, api_=api_, std_ratio=ratio or None,
+              model_bias_std={k: model_bias for k in BIAS_OPTIONS} if model_bias > 0 else None)
     if restart == "sample":
         if loop != "device":
             raise ValueError("--restart sample is an option of the device loop")
@@ -96,10 +104,10 @@ def gpu_info() -> dict:
 
 def run(n_env: int, steps: int, warmup: int, api_=None, robot: str = "atlas", loop: str = "host",
         duration_max: float = 0.4, disturbance: float = 0.0, sensors: float = 0.0, model: float = 0.0,
-        restart: str = "bank") -> dict:
+        restart: str = "bank", model_bias: float = 0.0) -> dict:
     import torch
     from jiminy_b200.envs import flatten_observation
-    env = make_env(n_env, api_, robot, loop, duration_max, disturbance, sensors, model, restart)
+    env = make_env(n_env, api_, robot, loop, duration_max, disturbance, sensors, model, restart, model_bias)
     device = loop == "device"
     on_gpu = device and env.torch_device.type == "cuda"
     nm = env.robot.nmotors
@@ -142,7 +150,7 @@ def run(n_env: int, steps: int, warmup: int, api_=None, robot: str = "atlas", lo
             f"contacts, euler_explicit 5 ms" if robot == "atlas" else
             f"{robot} PD standing (plain PD law), spring-damper contacts, runge_kutta_4 1 ms, per-step position targets")
     out = {"metric": "env_steps_per_sec", "unit": "env-steps/s", "value": n_env * steps / dt, "ms_per_step": 1e3 * dt / steps,
-           "loop": loop, "restart": restart, "robot": robot, "disturbance": disturbance, "sensors": sensors, "model": model, "n_env": n_env, "steps": steps, "warmup": warmup,
+           "loop": loop, "restart": restart, "robot": robot, "disturbance": disturbance, "sensors": sensors, "model": model, "model_bias": model_bias, "n_env": n_env, "steps": steps, "warmup": warmup,
            "timing": "host clock around env.step + flatten_observation, ending in a device synchronise",
            "config": {"workload": f"{desc}, {n_env} envs, step_dt {env.step_dt}, simulation_duration_max {duration_max}",
                       "env": type(env).__name__, "lane_plan": env.engine.describe(), "observation_width": int(flat.shape[1])},
@@ -172,8 +180,8 @@ def alternate(rounds: int, **kw) -> dict:
 
 
 def alternate_randomisation(rounds: int, ratios: dict, loops, **kw) -> dict:
-    """Each loop with the randomisation of `ratios` ({"disturbance": r}, {"sensors": r}, {"model": r}, or
-    {"restart": "sample"}) off and on, `rounds` times in this process, alternating; env-steps/s and spread."""
+    """Each loop with the randomisation of `ratios` ({"disturbance": r}, {"sensors": r}, {"model": r},
+    {"model_bias": s} or {"restart": "sample"}) off and on, `rounds` times in this process, alternating; env-steps/s and spread."""
     name = "_".join(ratios)
     runs = {(loop, on): [] for loop in loops for on in (False, True)}
     for _ in range(rounds):
@@ -204,11 +212,17 @@ if __name__ == "__main__":
     ap.add_argument("--disturbance", type=float, default=0.0, metavar="R")
     ap.add_argument("--sensors", type=float, default=0.0, metavar="R")
     ap.add_argument("--model", type=float, default=0.0, metavar="R")
+    ap.add_argument("--model-bias", type=float, default=0.0, metavar="S")
     ap.add_argument("--restart", choices=("bank", "sample"), default="bank")
     a = ap.parse_args()
     kw = dict(n_env=a.n_env, steps=a.steps, warmup=a.warmup, robot=a.robot, duration_max=a.duration_max)
     ratios = {k: r for k, r in (("disturbance", a.disturbance), ("sensors", a.sensors), ("model", a.model)) if r > 0}
-    if a.restart == "sample":
+    if a.model_bias > 0:
+        if a.restart == "sample":
+            kw["restart"] = "sample"
+        res = alternate_randomisation(max(a.alternate, 1), {"model_bias": a.model_bias},
+                                      (a.loop,), **ratios, **kw)
+    elif a.restart == "sample":
         res = alternate_randomisation(max(a.alternate, 1), {"restart": "sample"}, ("device",), **ratios, **kw)
     elif ratios:
         res = alternate_randomisation(max(a.alternate, 1), ratios, ("host", "device") if a.alternate > 0 else (a.loop,), **kw)
