@@ -493,6 +493,40 @@ int jb_set_model_env(JbBatch* batch, const uint8_t* mask, const double* rows);
 int jb_set_model_env_device(JbBatch* batch, const uint8_t* mask_dev, const double* rows_dev);
 int jb_get_model_env(JbBatch* batch, double* out);
 
+/* Reward and termination compositions: gym_jiminy's trajectory-free terms (jiminy_b200/compositions.py), evaluated per env
+ * on the device after every env-step, with no host synchronisation.
+ * jb_contact_positions_device enqueues the world position of every contact frame of every env from the accepted state,
+ * out_dev [n_env][ncontacts][3] (device memory), by the forward sweep of jb_start_device_on_ground on each env's own model
+ * (model variants, per-env model rows).  Envs that are not started or carry NaN read NaN.
+ * jb_set_compositions uploads the spec once (synchronising): n_node nodes, the reward tree first (n_reward nodes in
+ * post-order, root last), then the termination conditions in evaluation order.  Per node node_int [4] = kind
+ * (1 SurviveReward, 2 MinimizeMechanicalPowerConsumption, 3 AdditiveMixtureReward, 4 MultiplicativeMixtureReward,
+ * 10 BaseRollPitchTermination, 11 FallingTermination, 12 FlyingTermination, 13 MechanicalSafetyTermination,
+ * 14 MechanicalPowerConsumptionTermination), number of components (mixtures), EnergyGenerationMode (power terms),
+ * training_only; node_dbl [8] = grace_period, then the kind's numbers: power reward cutoff, horizon; additive order (inf
+ * allowed); roll-pitch low roll, low pitch, high roll, high pitch; falling low; flying high (at [3]); safety
+ * position_margin, velocity_max; power termination -, horizon (NaN: instantaneous), max_power (at [3]).  A NaN bound is
+ * not checked.  weights: the additive mixtures' weights in post-order, n_weight of them.  motor_int [nmotors][2] = q and
+ * v index of each motor's joint; motor_dbl [nmotors][3] = reduction, q_lower, q_upper of that joint.  env [3] = step_dt,
+ * simulation_duration_max, base height threshold (NaN: none).  A malformed or out-of-range spec (unknown kind or
+ * generator mode, a mixture without components, non-positive order, cutoff or horizon, negative or missing weights) is
+ * refused with JB_ERR_INVALID_ARGUMENT and nothing is uploaded.  Every env's power stacks are emptied.
+ * jb_compositions_device enqueues one launch.  restart_mask_dev null: evaluation after an env-step -- every power stack
+ * takes the power of the accepted state, then the env's own rule (base height, failure bits of the status word, time
+ * limit), the termination conditions (the first that fires wins) and the reward tree; writes reward [n_env],
+ * terminated / truncated [n_env] (0 / 1), index [2][n_env] (the condition that terminated / truncated, -1: none) and
+ * values [n_node][n_env] (each node's value, 1 / 0 for a condition that fired / did not, NaN: not evaluated).
+ * restart_mask_dev given: the masked envs' stacks are emptied and take the power of the state they (re)started from;
+ * nothing else is read or written.  The power uses the command held since the last controller update (the PD block's
+ * torque in PD mode, the command buffer otherwise). */
+int jb_contact_positions_device(JbBatch* batch, double* out_dev);
+int jb_set_compositions(JbBatch* batch, int32_t n_node, int32_t n_reward, const int32_t* node_int, const double* node_dbl,
+                        int32_t n_weight, const double* weights, const int32_t* motor_int, const double* motor_dbl,
+                        const double* env, int32_t training);
+int jb_compositions_device(JbBatch* batch, const uint8_t* restart_mask_dev, const int64_t* num_steps_dev,
+                           const double* contact_pos_dev, double* reward, uint8_t* terminated, uint8_t* truncated,
+                           int32_t* index, double* values);
+
 /* Stable zero-copy views of the state, like the `StepperState` / `RobotState` members the reference exposes to Python as
  * array views of the engine's own memory (python/jiminy_pywrap/include/jiminy/python/functors.h:57-68, generic.py:688-690:
  * a gym env reads `q`, `v`, the sensor matrix every step without a getter call).  The first call with `host` non-null

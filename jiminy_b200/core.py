@@ -70,7 +70,7 @@ class Api:
                "jb_set_sensor_options_env_device", "jb_set_seeds_device",
                "jb_enable_per_env_flexibility", "jb_set_flexibility_env", "jb_set_flexibility_env_device",
                "jb_get_flexibility_env", "jb_enable_per_env_model", "jb_set_model_env", "jb_set_model_env_device",
-               "jb_get_model_env")
+               "jb_get_model_env", "jb_contact_positions_device", "jb_set_compositions", "jb_compositions_device")
 
     def __init__(self, cdll: C.CDLL):
         self.dll = L = cdll
@@ -155,6 +155,10 @@ class Api:
         L.jb_set_model_env.argtypes = [vp, c_uint8_p, c_double_p]
         L.jb_set_model_env_device.argtypes = [vp, vp, vp]
         L.jb_get_model_env.argtypes = [vp, c_double_p]
+        L.jb_contact_positions_device.argtypes = [vp, vp]
+        L.jb_set_compositions.argtypes = [vp, C.c_int32, C.c_int32, c_int32_p, c_double_p, C.c_int32, c_double_p, c_int32_p,
+                                          c_double_p, c_double_p, C.c_int32]
+        L.jb_compositions_device.argtypes = [vp] * 9
 
     def check(self, rc: int) -> None:
         if rc != JB_OK:
@@ -625,6 +629,31 @@ class BatchedEngine:
         """The robot table env `env` runs with: the batch's robot with that env's inertias and joint-placement
         translations (`get_model_env`)."""
         return M.with_body_rows(self.robot, self.get_model_env()[env])
+
+    # ---- reward and termination compositions (jiminy_b200.compositions)
+    def contact_positions_device(self, out_ptr: int) -> None:
+        """Enqueues the world position of every contact frame of every env, from the accepted state and each env's own
+        model, into the device buffer `out_ptr` [n_env, ncontacts, 3] (fp64).  Not started / NaN envs read NaN."""
+        self._api.check(self._api.dll.jb_contact_positions_device(self._h, C.c_void_p(out_ptr)))
+
+    def set_compositions(self, node_int, node_dbl, n_reward: int, weights, motor_int, motor_dbl, env, training: bool) -> None:
+        """Uploads a composition spec (`compositions.Spec` gives the arrays; layout in include/jiminy_b200.h) and empties
+        every env's power stacks.  A malformed spec raises ValueError and nothing is uploaded."""
+        ni, nd = np.ascontiguousarray(node_int, dtype=np.int32), np.ascontiguousarray(node_dbl, dtype=np.float64)
+        w = np.ascontiguousarray(weights, dtype=np.float64)
+        mi, md = np.ascontiguousarray(motor_int, dtype=np.int32), np.ascontiguousarray(motor_dbl, dtype=np.float64)
+        e = np.ascontiguousarray(env, dtype=np.float64)
+        self._api.check(self._api.dll.jb_set_compositions(
+            self._h, len(ni), n_reward, ni.ctypes.data_as(c_int32_p), dptr(nd), len(w), dptr(w) if len(w) else None,
+            mi.ctypes.data_as(c_int32_p) if len(mi) else None, dptr(md) if len(md) else None, dptr(e), int(bool(training))))
+
+    def compositions_device(self, restart_mask_ptr: Optional[int] = None, num_steps_ptr: int = 0, contact_ptr: int = 0,
+                            reward_ptr: int = 0, terminated_ptr: int = 0, truncated_ptr: int = 0, index_ptr: int = 0,
+                            values_ptr: int = 0) -> None:
+        """Enqueues one launch of the composition kernel (see include/jiminy_b200.h): the evaluation after an env-step,
+        or, with `restart_mask_ptr`, the reseeding of the power stacks of the envs that have just (re)started."""
+        ptrs = (restart_mask_ptr, num_steps_ptr, contact_ptr, reward_ptr, terminated_ptr, truncated_ptr, index_ptr, values_ptr)
+        self._api.check(self._api.dll.jb_compositions_device(self._h, *(C.c_void_p(p or None) for p in ptrs)))
 
     def get_sensor_data(self) -> np.ndarray:
         out = np.zeros((self.n_env, max(self.width, 1)))

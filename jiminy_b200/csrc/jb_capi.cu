@@ -130,6 +130,14 @@ struct JbBatch {
     std::vector<int32_t> h_joint_parent, h_pem_row, h_pem_massless;
     double *d_pem_pending = nullptr, *d_pem_stage = nullptr;
     int32_t* d_pem_massless = nullptr;
+    // reward and termination compositions (jb_set_compositions): spec [n][COMP_INT_W] / [n][COMP_DBL_W], mixture weights,
+    // motor table, per-env power stacks [n_env][comp_stack_w] and push counts [n_env][n]
+    int ncontacts = 0;
+    int32_t comp_n = 0, comp_n_reward = 0, comp_stack_w = 0, comp_training = 0;
+    double comp_env[3] = {0.0, 0.0, 0.0};   // step_dt, simulation_duration_max, height_min (NaN: none)
+    int32_t *d_comp_int = nullptr, *d_comp_motor_int = nullptr, *d_comp_count = nullptr;
+    double *d_comp_dbl = nullptr, *d_comp_w = nullptr, *d_comp_motor_dbl = nullptr, *d_comp_stack = nullptr;
+    size_t comp_cap[7] = {};
 };
 
 // The dynamic shared-memory opt-in is a per-function, per-device attribute: only ever raise it.
@@ -147,6 +155,7 @@ static int raise_smem_attr(int device, size_t bytes) {
     if (e == cudaSuccess) e = cudaFuncSetAttribute(env_step_kernel_model_ext, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(bytes));
     if (e == cudaSuccess) e = cudaFuncSetAttribute(env_step_kernel_model, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(bytes));
     if (e == cudaSuccess) e = cudaFuncSetAttribute(env_step_kernel_model_flex, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(bytes));
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(contact_positions_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(bytes));
     if (e != cudaSuccess) return fail(JB_ERR_CUDA, std::string("cudaFuncSetAttribute: ") + cudaGetErrorString(e));
     g_smem_attr[device] = bytes;
 #endif
@@ -214,10 +223,7 @@ static int ensure_host_stage(JbBatch* b, size_t bytes) {
     return JB_OK;
 }
 
-// One launch of the step kernel.  The persistent parameter block lives in constant memory, one per device: it is
-// re-uploaded only when it differs from what the device holds (another batch launched in between, or a setter
-// changed it), ordered after every earlier launch on that device.  What changes at every launch (mode, step size,
-// peer-exchange step) travels as the kernel parameter.
+// The parameter block each device holds in constant memory (with_params)
 #ifndef JB_HOST_EMUL
 static KParams g_kp_on_device[64];
 static bool g_kp_valid[64] = {};
@@ -262,6 +268,42 @@ __global__ void latch_model_rows_kernel(RecDbl* __restrict__ tables, double* __r
     }
 }
 
+// Makes the device's parameter block this batch's `kp`, then enqueues `go` (a launch reading KP) on the batch stream.
+// The block lives in constant memory, one per device: it is re-uploaded only when it differs from what the device holds
+// (another batch launched in between, or a setter changed it), ordered after every earlier launch on that device.
+// `mirrors`: a launch of the step kernel that changes the state, refreshed into the jb_state_ptrs mirrors behind it.
+static int refresh_mirrors(JbBatch* b);
+template <class F>
+static int with_params(JbBatch* b, const KParams& kp, F&& go, bool mirrors = false) {
+#ifdef JB_HOST_EMUL
+    emul::current_L = b->plan.L;
+    g_kp_host = kp;
+    go();
+#else
+    {
+        std::lock_guard<std::mutex> lock(g_launch_mutex);
+        cudaEvent_t& evt = g_last_launch[b->device];
+        if (!evt) CU(cudaEventCreateWithFlags(&evt, cudaEventDisableTiming));
+        if (!g_kp_valid[b->device] || std::memcmp(&g_kp_on_device[b->device], &kp, sizeof kp) != 0) {
+            if (g_kp_valid[b->device]) CU(cudaStreamWaitEvent(b->stream, evt, 0));
+            g_kp_valid[b->device] = false;
+            // (the copy is staged by the runtime before the call returns: `kp` may live on this stack)
+            CU(cudaMemcpyToSymbolAsync(g_kp, &kp, sizeof kp, 0, cudaMemcpyHostToDevice, b->stream));
+            std::memcpy(&g_kp_on_device[b->device], &kp, sizeof kp);
+            g_kp_valid[b->device] = true;
+            ++b->param_uploads;
+        }
+        go();
+        CU(cudaEventRecord(evt, b->stream));
+    }
+#endif
+    CU(cudaGetLastError());
+    ++b->launches;
+    return mirrors ? refresh_mirrors(b) : JB_OK;
+}
+
+// One launch of the step kernel.  What changes at every launch (mode, step size, peer-exchange step) travels as the
+// kernel parameter.
 static int launch(JbBatch* b, int mode, double step_dt, const uint8_t* d_mask = nullptr, const double* d_command = nullptr,
                   bool validate = false, bool ground = false) {
     KParams kp = b->kp;
@@ -292,33 +334,7 @@ static int launch(JbBatch* b, int mode, double step_dt, const uint8_t* d_mask = 
         CU(cudaGetLastError());
         ++b->launches;
     }
-#ifdef JB_HOST_EMUL
-    emul::current_L = b->plan.L;
-    g_kp_host = kp;
-    if (kp.pem_on) {
-        if (kp.flex_on) JB_LAUNCH(env_step_kernel_model_flex, nblocks, 32, b->smem_bytes, b->stream, la);
-        else if (fast) JB_LAUNCH(env_step_kernel_model_fast, nblocks, 32, b->smem_bytes, b->stream, la);
-        else if (fast_ext) JB_LAUNCH(env_step_kernel_model_ext, nblocks, 32, b->smem_bytes, b->stream, la);
-        else JB_LAUNCH(env_step_kernel_model, nblocks, 32, b->smem_bytes, b->stream, la);
-    }
-    else if (kp.flex_on) JB_LAUNCH(env_step_kernel_flex, nblocks, 32, b->smem_bytes, b->stream, la);
-    else if (fast) JB_LAUNCH(env_step_kernel_t<true>, nblocks, 32, b->smem_bytes, b->stream, la);
-    else if (fast_ext) JB_LAUNCH(env_step_kernel_ext, nblocks, 32, b->smem_bytes, b->stream, la);
-    else JB_LAUNCH(env_step_kernel_t<false>, nblocks, 32, b->smem_bytes, b->stream, la);
-#else
-    {
-        std::lock_guard<std::mutex> lock(g_launch_mutex);
-        cudaEvent_t& evt = g_last_launch[b->device];
-        if (!evt) CU(cudaEventCreateWithFlags(&evt, cudaEventDisableTiming));
-        if (!g_kp_valid[b->device] || std::memcmp(&g_kp_on_device[b->device], &kp, sizeof kp) != 0) {
-            if (g_kp_valid[b->device]) CU(cudaStreamWaitEvent(b->stream, evt, 0));
-            g_kp_valid[b->device] = false;
-            // (the copy is staged by the runtime before the call returns: `kp` may live on this stack)
-            CU(cudaMemcpyToSymbolAsync(g_kp, &kp, sizeof kp, 0, cudaMemcpyHostToDevice, b->stream));
-            std::memcpy(&g_kp_on_device[b->device], &kp, sizeof kp);
-            g_kp_valid[b->device] = true;
-            ++b->param_uploads;
-        }
+    return with_params(b, kp, [&]() {
         if (kp.pem_on) {
             if (kp.flex_on) JB_LAUNCH(env_step_kernel_model_flex, nblocks, 32, b->smem_bytes, b->stream, la);
             else if (fast) JB_LAUNCH(env_step_kernel_model_fast, nblocks, 32, b->smem_bytes, b->stream, la);
@@ -329,12 +345,12 @@ static int launch(JbBatch* b, int mode, double step_dt, const uint8_t* d_mask = 
         else if (fast) JB_LAUNCH(env_step_kernel_t<true>, nblocks, 32, b->smem_bytes, b->stream, la);
         else if (fast_ext) JB_LAUNCH(env_step_kernel_ext, nblocks, 32, b->smem_bytes, b->stream, la);
         else JB_LAUNCH(env_step_kernel_t<false>, nblocks, 32, b->smem_bytes, b->stream, la);
-        CU(cudaEventRecord(evt, b->stream));
-    }
-#endif
-    CU(cudaGetLastError());
-    ++b->launches;
-    if (b->h_mirror && (mode == MODE_STEP || mode == MODE_START)) {
+    }, mode == MODE_STEP || mode == MODE_START);
+}
+
+// After a launch of the step kernel: mirrors of the state for jb_state_ptrs
+static int refresh_mirrors(JbBatch* b) {
+    if (b->h_mirror) {
         // behind the step on the same stream: the views hold the new state once the stream has been synchronised
         CU(cudaMemcpyAsync(b->hm_t, b->d_sched + static_cast<size_t>(SCH_T) * b->n_pad, sizeof(double) * b->n_env, cudaMemcpyDeviceToHost, b->stream));
         CU(cudaMemcpyAsync(b->hm_qv, b->d_qv, sizeof(double) * b->n_env * (b->nq + b->nv), cudaMemcpyDeviceToHost, b->stream));
@@ -449,6 +465,7 @@ int jb_batch_create(const JbModelDesc* m, const JbOptions* opt, int32_t n_env, i
     const Plan& P = b->plan;
     if (P.nrec > MAX_REC) { delete b; return fail(JB_ERR_NOT_IMPLEMENTED, "too many records per lane"); }
     b->nq = m->nq; b->nv = m->nv; b->nmotors = m->nmotors; b->njoints = m->njoints; b->nimu = m->nimu;
+    b->ncontacts = m->ncontacts;
     b->q_lower.assign(m->q_lower, m->q_lower + m->nq);
     b->q_upper.assign(m->q_upper, m->q_upper + m->nq);
     if (cudaStreamCreateWithFlags(&b->stream, cudaStreamNonBlocking) != cudaSuccess) { delete b; return fail(JB_ERR_CUDA, "stream creation failed"); }
@@ -2338,6 +2355,295 @@ int jb_debug_prof(JbBatch* b, double* out16) {
     return JB_OK;
 }
 #endif
+
+// ---- reward and termination compositions (gym_jiminy's trajectory-free terms) -----------------------------------------
+// Spec node: ints [kind, n_children, generator_mode, training_only, stack offset, max_stack] (the last two filled here),
+// doubles [grace_period, a1, a2, a3, a4, 0, 0, 0].  Nodes 0 .. n_reward-1 are the reward tree in post-order, the others
+// the termination conditions in evaluation order.  What jiminy_b200/compositions.py restates on the host, operation for
+// operation: products and sums without contraction into FMAs (JB_MUL_RN / JB_ADD_RN).  Only pow (the RBF transform and an
+// L^p mixture of order other than 1, or a geometric mean) and sin / cos / atan2 (roll and pitch) come from the device's
+// math library and may differ from the host's by a few ulp.
+constexpr int COMP_INT_W = 6, COMP_DBL_W = 8, COMP_IN_INT_W = 4, COMP_MAX_NODES = 32;
+enum : int32_t { COMP_SURVIVE = 1, COMP_POWER = 2, COMP_ADDITIVE = 3, COMP_MULTIPLICATIVE = 4,
+                 TERM_ROLL_PITCH = 10, TERM_FALLING = 11, TERM_FLYING = 12, TERM_SAFETY = 13, TERM_POWER = 14 };
+
+struct CompArgs {
+    const int32_t* node_int; const double* node_dbl; const double* weights;
+    const int32_t* motor_int; const double* motor_dbl;    // [nm][2] idx_q idx_v, [nm][3] reduction q_lower q_upper
+    const double* t; const double* qv; const double* command; const int32_t* status;
+    const long long* num_steps; const double* contact_pos; const uint8_t* mask;
+    double* stack; int32_t* count;
+    double* reward; uint8_t* terminated; uint8_t* truncated; int32_t* index; double* values;
+    int32_t n_node, n_reward, nm, ncontacts, nq, nv, n_env, stack_w, training;
+    double step_dt, t_max, height_min;
+};
+
+// compute_power (quantities/generic.py): motor-side velocity times the held command, summed motor after motor
+__device__ __forceinline__ double comp_power(const CompArgs& a, int mode, const double* v, const double* cmd) {
+    double s = 0.0;
+    for (int m = 0; m < a.nm; ++m) {
+        const double p = JB_MUL_RN(JB_MUL_RN(v[a.motor_int[2 * m + 1]], a.motor_dbl[3 * m]), cmd[m]);
+        s = JB_ADD_RN(s, mode == 1 ? (p < 0.0 ? 0.0 : p) : (mode == 3 ? fabs(p) : p));
+    }
+    return (mode == 2 && s < 0.0) ? 0.0 : s;
+}
+
+// mean of a node's power stack, oldest entry first
+__device__ __forceinline__ double comp_stack_mean(const CompArgs& a, const double* st, int32_t cnt, int M) {
+    const int n = cnt < M ? cnt : M, first = cnt < M ? 0 : cnt % M;
+    double s = 0.0;
+    for (int k = 0; k < n; ++k) s = JB_ADD_RN(s, st[(first + k) % M]);
+    return s / n;
+}
+
+// One thread per env.  Seed launch (a.mask given): the masked envs' stacks are cleared and get the power of the state
+// they (re)started from.  Evaluation launch: push the power of the accepted state, then the env's own rule, the
+// termination conditions (first that fires wins) and the reward tree, as ComposedJiminyEnv does after an env-step.
+__global__ void compositions_kernel(const CompArgs a) {
+    const int e = blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= a.n_env) return;
+    const double* q = a.qv + static_cast<size_t>(e) * (a.nq + a.nv);
+    const double* v = q + a.nq;
+    const double* cmd = a.command + static_cast<size_t>(e) * a.nm;
+    double* const stack = a.stack + static_cast<size_t>(e) * a.stack_w;
+    int32_t* const count = a.count + static_cast<size_t>(e) * a.n_node;
+    const size_t N = a.n_env;
+    for (int i = 0; i < a.n_node; ++i) {
+        const int32_t* ni = a.node_int + i * COMP_INT_W;
+        if (ni[5] == 0) continue;
+        if (a.mask && !a.mask[e]) continue;
+        const int32_t cnt = a.mask ? 0 : count[i];
+        stack[ni[4] + cnt % ni[5]] = comp_power(a, ni[2], v, cmd);
+        count[i] = cnt + 1;
+    }
+    if (a.mask) return;
+    // envs.terminated_truncated
+    const int32_t status = a.status[e];
+    bool truncated = (status & ~JB_ENV_JOINT_LIMIT) != 0 || static_cast<double>(a.num_steps[e]) * a.step_dt >= a.t_max;
+    bool terminated = a.height_min == a.height_min && q[2] < a.height_min;
+    int32_t fired = -1;
+    const bool base_done = terminated || truncated;
+    for (int i = a.n_reward; i < a.n_node; ++i) {
+        const int32_t* ni = a.node_int + i * COMP_INT_W;
+        const double* nd = a.node_dbl + i * COMP_DBL_W;
+        double value = D_NAN;
+        if (!base_done && fired < 0) {
+            bool hit = false;
+            if (!((ni[3] && !a.training) || a.t[e] < nd[0])) {
+                const double lo = nd[1], hi = nd[3];
+                if (ni[0] == TERM_ROLL_PITCH) {
+                    // pinocchio's quaternion -> rotation matrix, then matrix_to_rpy (utils/math.py)
+                    const double x = q[3], y = q[4], z = q[5], w = q[6];
+                    const double tx = JB_ADD_RN(x, x), ty = JB_ADD_RN(y, y), tz = JB_ADD_RN(z, z);
+                    const double twx = JB_MUL_RN(tx, w), twy = JB_MUL_RN(ty, w), twz = JB_MUL_RN(tz, w);
+                    const double txx = JB_MUL_RN(tx, x), txy = JB_MUL_RN(ty, x), txz = JB_MUL_RN(tz, x);
+                    const double tyy = JB_MUL_RN(ty, y), tyz = JB_MUL_RN(tz, y), tzz = JB_MUL_RN(tz, z);
+                    const double R00 = 1.0 - JB_ADD_RN(tyy, tzz), R01 = txy - twz, R02 = JB_ADD_RN(txz, twy);
+                    const double R10 = JB_ADD_RN(txy, twz), R11 = 1.0 - JB_ADD_RN(txx, tzz), R12 = tyz - twx;
+                    const double R20 = txz - twy, R21 = JB_ADD_RN(tyz, twx), R22 = 1.0 - JB_ADD_RN(txx, tyy);
+                    const double cp = sqrt(JB_ADD_RN(JB_MUL_RN(R22, R22), JB_MUL_RN(R21, R21)));
+                    const double pitch = atan2(-R20, cp), yaw = atan2(R10, R00);
+                    const double sy = sin(yaw), cy = cos(yaw);
+                    const double roll = atan2(JB_MUL_RN(sy, R02) - JB_MUL_RN(cy, R12), JB_MUL_RN(cy, R11) - JB_MUL_RN(sy, R01));
+                    // array bounds (_array_contains): out unless lo <= x <= hi, so NaN is out
+                    hit = (lo == lo && !(lo <= roll)) || (nd[2] == nd[2] && !(nd[2] <= pitch)) ||
+                          (hi == hi && !(roll <= hi)) || (nd[4] == nd[4] && !(pitch <= nd[4]));
+                } else if (ni[0] == TERM_SAFETY) {
+                    for (int m = 0; m < a.nm; ++m) {
+                        const double qj = q[a.motor_int[2 * m]], vj = v[a.motor_int[2 * m + 1]];
+                        const double* md = a.motor_dbl + 3 * m;
+                        hit = hit || ((qj - md[1] < nd[1]) && (vj < -nd[2])) || ((md[2] - qj < nd[1]) && (vj > nd[2]));
+                    }
+                } else {
+                    double x;
+                    if (ni[0] == TERM_POWER) x = ni[5] ? comp_stack_mean(a, stack + ni[4], count[i], ni[5]) : comp_power(a, ni[2], v, cmd);
+                    else {
+                        double zmin = D_INF;
+                        const double* cpos = a.contact_pos + static_cast<size_t>(e) * a.ncontacts * 3;
+                        for (int k = 0; k < a.ncontacts; ++k) { const double zk = cpos[3 * k + 2]; zmin = (zk < zmin || zk != zk) ? zk : zmin; }
+                        x = ni[0] == TERM_FALLING ? q[2] - zmin : zmin;
+                    }
+                    // scalar bounds (_array_contains): out if lo > x or x > hi, so NaN is in
+                    hit = (lo == lo && lo > x) || (hi == hi && x > hi);
+                }
+            }
+            value = hit ? 1.0 : 0.0;
+            if (hit) { fired = i - a.n_reward; terminated = true; }
+        }
+        a.values[i * N + e] = value;
+    }
+    // the reward tree, post-order: a non-terminal term is not evaluated on a terminal step; a mixture skips the
+    // components that were not, and is not evaluated itself when none was
+    double val[COMP_MAX_NODES];
+    bool ok[COMP_MAX_NODES];
+    int sp = 0, wk = 0;
+    for (int i = 0; i < a.n_reward; ++i) {
+        const int32_t* ni = a.node_int + i * COMP_INT_W;
+        const double* nd = a.node_dbl + i * COMP_DBL_W;
+        double x = 0.0;
+        bool has = false;
+        if (ni[0] == COMP_SURVIVE) { x = 1.0; has = !terminated; }
+        else if (ni[0] == COMP_POWER) {
+            if (!terminated) {
+                const double p = comp_stack_mean(a, stack + ni[4], count[i], ni[5]);
+                x = pow(0.01, JB_MUL_RN(p, p) / JB_MUL_RN(nd[1], nd[1]));   // radial_basis_function(order=2), CUTOFF_ESP
+                has = true;
+            }
+        } else {
+            const int k = ni[1];
+            sp -= k;
+            if (ni[0] == COMP_ADDITIVE) {
+                const double order = nd[1];
+                const bool inf = order > 1.7976931348623157e308;
+                for (int j = 0; j < k; ++j) {
+                    if (!ok[sp + j]) continue;
+                    const double w = a.weights[wk + j], y = val[sp + j];
+                    if (inf) { const double wy = JB_MUL_RN(w, y); x = (!has || wy > x) ? wy : x; }   // Python's max(x, wy)
+                    else x = JB_ADD_RN(x, JB_MUL_RN(w, order == 1.0 ? y : pow(y, order)));
+                    has = true;
+                }
+                if (has && !inf && order != 1.0) x = pow(x, 1.0 / order);
+                wk += k;
+            } else {
+                int n = 0;
+                x = 1.0;
+                for (int j = 0; j < k; ++j) if (ok[sp + j]) { x = JB_MUL_RN(x, val[sp + j]); ++n; }
+                has = n > 0;
+                if (has && n != 1) x = pow(x, 1.0 / n);
+            }
+        }
+        val[sp] = x; ok[sp] = has; ++sp;
+        a.values[i * N + e] = has ? x : D_NAN;
+    }
+    a.reward[e] = ok[0] ? val[0] : 0.0;
+    a.terminated[e] = terminated ? 1 : 0;
+    a.truncated[e] = truncated ? 1 : 0;
+    a.index[e] = fired;     // info["terminated"]: every supported condition terminates
+    a.index[N + e] = -1;    // info["truncated"]
+}
+
+int jb_set_compositions(JbBatch* b, int32_t n_node, int32_t n_reward, const int32_t* node_int, const double* node_dbl,
+                        int32_t n_weight, const double* weights, const int32_t* motor_int, const double* motor_dbl,
+                        const double* env, int32_t training) {
+    if (!b || !node_int || !node_dbl || !env || (n_weight > 0 && !weights) || (b->nmotors > 0 && (!motor_int || !motor_dbl)))
+        return fail(JB_ERR_INVALID_ARGUMENT, "null argument");
+    if (n_reward < 1 || n_node < n_reward || n_node > COMP_MAX_NODES)
+        return fail(JB_ERR_INVALID_ARGUMENT, "compositions: 1 to " + std::to_string(COMP_MAX_NODES) + " nodes, the reward tree first");
+    const double step_dt = env[0];
+    if (!(step_dt > 0.0) || !std::isfinite(step_dt)) return fail(JB_ERR_INVALID_ARGUMENT, "compositions: step_dt must be positive");
+    std::vector<int32_t> ni(static_cast<size_t>(n_node) * COMP_INT_W, 0);
+    std::vector<double> nd(node_dbl, node_dbl + static_cast<size_t>(n_node) * COMP_DBL_W);
+    int depth = 0, nw = 0, stack_w = 0;
+    for (int i = 0; i < n_node; ++i) {
+        const int32_t* in = node_int + i * COMP_IN_INT_W;
+        const double* d = node_dbl + i * COMP_DBL_W;
+        int32_t* o = ni.data() + i * COMP_INT_W;
+        for (int k = 0; k < COMP_IN_INT_W; ++k) o[k] = in[k];
+        const int kind = in[0];
+        const std::string where = "compositions: node " + std::to_string(i) + ": ";
+        const bool reward = i < n_reward;
+        const bool leaf = kind == COMP_SURVIVE || kind == COMP_POWER;
+        const bool mixture = kind == COMP_ADDITIVE || kind == COMP_MULTIPLICATIVE;
+        const bool term = kind >= TERM_ROLL_PITCH && kind <= TERM_POWER;
+        if (reward ? !(leaf || mixture) : !term) return fail(JB_ERR_INVALID_ARGUMENT, where + "unknown kind " + std::to_string(kind));
+        if ((kind == COMP_POWER || kind == TERM_POWER) && (in[2] < 0 || in[2] > 3))
+            return fail(JB_ERR_INVALID_ARGUMENT, where + "unknown generator mode");
+        if (term && !(d[0] >= 0.0 && std::isfinite(d[0]))) return fail(JB_ERR_INVALID_ARGUMENT, where + "grace period must be finite and >= 0");
+        double horizon = std::nan("");
+        if (kind == COMP_POWER) {
+            if (!(d[1] > 0.0) || !std::isfinite(d[1])) return fail(JB_ERR_INVALID_ARGUMENT, where + "cutoff must be positive");
+            horizon = d[2];
+            if (!(horizon > 0.0) || !std::isfinite(horizon)) return fail(JB_ERR_INVALID_ARGUMENT, where + "horizon must be positive");
+        }
+        if (kind == TERM_POWER) {
+            horizon = d[2];
+            if (horizon == horizon && (!(horizon > 0.0) || !std::isfinite(horizon)))
+                return fail(JB_ERR_INVALID_ARGUMENT, where + "horizon must be positive");
+        }
+        if (kind == TERM_SAFETY && !(d[1] == d[1] && d[2] == d[2])) return fail(JB_ERR_INVALID_ARGUMENT, where + "margin and velocity must be numbers");
+        if (horizon == horizon) {
+            // StackedQuantity of AverageMechanicalPowerConsumption: max(ceil(horizon / step_dt), 1) + 1 entries
+            const int M = std::max(static_cast<int>(std::ceil(horizon / step_dt)), 1) + 1;
+            if (M > (1 << 16)) return fail(JB_ERR_INVALID_ARGUMENT, where + "horizon over 65535 env-steps");
+            o[4] = stack_w; o[5] = M; stack_w += M;
+        }
+        if (mixture) {
+            if (in[1] < 1 || in[1] > depth) return fail(JB_ERR_INVALID_ARGUMENT, where + "mixture without its components (post-order)");
+            depth -= in[1];
+            if (kind == COMP_ADDITIVE) {
+                if (!(d[1] > 0.0)) return fail(JB_ERR_INVALID_ARGUMENT, where + "'order' must be strictly positive or 'inf'.");
+                if (nw + in[1] > n_weight) return fail(JB_ERR_INVALID_ARGUMENT, where + "Exactly one weight per reward component must be specified.");
+                for (int k = 0; k < in[1]; ++k)
+                    if (!(weights[nw + k] >= 0.0) || !std::isfinite(weights[nw + k])) return fail(JB_ERR_INVALID_ARGUMENT, where + "weights must be finite and >= 0");
+                nw += in[1];
+            }
+        } else if (in[1] != 0) return fail(JB_ERR_INVALID_ARGUMENT, where + "only mixtures have components");
+        if (reward) ++depth;
+    }
+    if (depth != 1) return fail(JB_ERR_INVALID_ARGUMENT, "compositions: the reward nodes are not one tree in post-order");
+    if (nw != n_weight) return fail(JB_ERR_INVALID_ARGUMENT, "compositions: Exactly one weight per reward component must be specified.");
+    for (int m = 0; m < b->nmotors; ++m)
+        if (motor_int[2 * m] < 0 || motor_int[2 * m] >= b->nq || motor_int[2 * m + 1] < 0 || motor_int[2 * m + 1] >= b->nv)
+            return fail(JB_ERR_INVALID_ARGUMENT, "compositions: motor table index out of range");
+    CU(cudaSetDevice(b->device));
+    const size_t n = b->n_env, nm = std::max(b->nmotors, 1);
+    int rc = dev_reserve(b, &b->d_comp_int, &b->comp_cap[0], ni.size());
+    if (!rc) rc = dev_reserve(b, &b->d_comp_dbl, &b->comp_cap[1], nd.size());
+    if (!rc) rc = dev_reserve(b, &b->d_comp_w, &b->comp_cap[2], std::max(n_weight, 1));
+    if (!rc) rc = dev_reserve(b, &b->d_comp_motor_int, &b->comp_cap[3], 2 * nm);
+    if (!rc) rc = dev_reserve(b, &b->d_comp_motor_dbl, &b->comp_cap[4], 3 * nm);
+    if (!rc) rc = dev_reserve(b, &b->d_comp_stack, &b->comp_cap[5], n * std::max(stack_w, 1));
+    if (!rc) rc = dev_reserve(b, &b->d_comp_count, &b->comp_cap[6], n * n_node);
+    if (rc) return rc;
+    CU(cudaMemcpyAsync(b->d_comp_int, ni.data(), ni.size() * sizeof(int32_t), cudaMemcpyHostToDevice, b->stream));
+    CU(cudaMemcpyAsync(b->d_comp_dbl, nd.data(), nd.size() * sizeof(double), cudaMemcpyHostToDevice, b->stream));
+    if (n_weight) CU(cudaMemcpyAsync(b->d_comp_w, weights, n_weight * sizeof(double), cudaMemcpyHostToDevice, b->stream));
+    if (b->nmotors) {
+        CU(cudaMemcpyAsync(b->d_comp_motor_int, motor_int, 2 * b->nmotors * sizeof(int32_t), cudaMemcpyHostToDevice, b->stream));
+        CU(cudaMemcpyAsync(b->d_comp_motor_dbl, motor_dbl, 3 * b->nmotors * sizeof(double), cudaMemcpyHostToDevice, b->stream));
+    }
+    CU(cudaMemsetAsync(b->d_comp_count, 0, n * n_node * sizeof(int32_t), b->stream));
+    CU(cudaStreamSynchronize(b->stream));
+    b->comp_n = n_node; b->comp_n_reward = n_reward; b->comp_stack_w = stack_w; b->comp_training = training ? 1 : 0;
+    b->comp_env[0] = step_dt; b->comp_env[1] = env[1]; b->comp_env[2] = env[2];
+    return JB_OK;
+}
+
+int jb_contact_positions_device(JbBatch* b, double* out_dev) {
+    if (!b || !out_dev) return fail(JB_ERR_INVALID_ARGUMENT, "null argument");
+    if (b->ncontacts == 0) return JB_OK;
+    CU(cudaSetDevice(b->device));
+    KParams kp = b->kp;
+    if (kp.n_eslot > 0) kp.sig_id = 0;     // as launch(): the parameter block the full body reads
+    const int epw = 32 / b->plan.L;
+    const int nblocks = (b->n_env + epw - 1) / epw;
+    const int nc = b->ncontacts;
+    return with_params(b, kp, [&]() { JB_LAUNCH(contact_positions_kernel, nblocks, 32, b->smem_bytes, b->stream, out_dev, nc); });
+}
+
+int jb_compositions_device(JbBatch* b, const uint8_t* restart_mask_dev, const int64_t* num_steps_dev, const double* contact_pos_dev,
+                           double* reward, uint8_t* terminated, uint8_t* truncated, int32_t* index, double* values) {
+    if (!b) return fail(JB_ERR_INVALID_ARGUMENT, "null argument");
+    if (b->comp_n == 0) return fail(JB_ERR_BAD_CONTROL_FLOW, "no compositions set (jb_set_compositions)");
+    if (!restart_mask_dev && (!num_steps_dev || (!contact_pos_dev && b->ncontacts) || !reward || !terminated || !truncated || !index || !values))
+        return fail(JB_ERR_INVALID_ARGUMENT, "null argument");
+    CU(cudaSetDevice(b->device));
+    CompArgs a{};
+    a.node_int = b->d_comp_int; a.node_dbl = b->d_comp_dbl; a.weights = b->d_comp_w;
+    a.motor_int = b->d_comp_motor_int; a.motor_dbl = b->d_comp_motor_dbl;
+    a.t = b->d_sched + static_cast<size_t>(SCH_T) * b->n_pad; a.qv = b->d_qv;
+    a.command = (b->kp.pd_gains || b->kp.pdf) ? b->d_cmd_torque : b->d_cmd;     // the command held since the last update
+    a.status = b->d_status; a.num_steps = reinterpret_cast<const long long*>(num_steps_dev); a.contact_pos = contact_pos_dev;
+    a.mask = restart_mask_dev; a.stack = b->d_comp_stack; a.count = b->d_comp_count;
+    a.reward = reward; a.terminated = terminated; a.truncated = truncated; a.index = index; a.values = values;
+    a.n_node = b->comp_n; a.n_reward = b->comp_n_reward; a.nm = b->nmotors; a.ncontacts = b->ncontacts; a.nq = b->nq; a.nv = b->nv;
+    a.n_env = b->n_env; a.stack_w = b->comp_stack_w; a.training = b->comp_training;
+    a.step_dt = b->comp_env[0]; a.t_max = b->comp_env[1]; a.height_min = b->comp_env[2];
+    JB_LAUNCH(compositions_kernel, static_cast<unsigned>((b->n_env + 127) / 128), 128, 0, b->stream, a);
+    CU(cudaGetLastError());
+    ++b->launches;
+    return JB_OK;
+}
 
 int jb_synchronize(JbBatch* b) {
     if (!b) return fail(JB_ERR_INVALID_ARGUMENT, "null argument");

@@ -21,6 +21,7 @@ namespace jb {
 constexpr int MAX_REC = 48;
 constexpr double D_EPS = 2.220446049250313e-16;
 #define D_INF (__longlong_as_double(0x7ff0000000000000LL))
+#define D_NAN (__longlong_as_double(0x7ff8000000000000LL))
 constexpr double STEPPER_MIN_TIMESTEP = 1e-10;   // core/include/jiminy/core/constants.h:18-20
 constexpr double SIMULATION_MIN_TIMESTEP = 1e-6;
 

@@ -78,26 +78,13 @@ JB_DI void normalize_record(const Ctx& c, const RecInt* ri, int base) {
     }
 }
 
-// jb_start_device_on_ground: `robots.ground_base_height` on the device (the rule of BaseJiminyEnv._sample_state,
-// generic.py:1300-1335): q[2] of this env's input row is lowered or raised so that its lowest contact frame touches the
-// flat ground z = 0.  The forward kinematics runs on the row as given (before the start's quaternion normalisation), with
-// the forward sweep's joint transforms (joint_calc) and this block's model variant.  Each lane takes the min over its own
-// contact slots, then every lane reads the group's lane minima in the order 0 .. L-1, so that all of them agree bit for
-// bit.  Sub-lane 0 writes q[2] into the batch's own copy of the row (KP->q_in), which the input checks and the loads of
-// the start then read.  The min keeps a NaN, so a row that yields one still fails the checks.  Without a free-flyer at
-// q[0:7] or without a contact frame the row is left as it is.
-__device__ __noinline__ void place_on_ground(const Ctx c) {
+// Forward sweep of the lane's records from the loaded positions, with the step's joint transforms (joint_calc), pool
+// transforms and contact slots: on_contact(slot, world position) for every contact slot of the lane.  Shared by the
+// grounding of a start (place_on_ground) and the contact-frame pass (contact_positions_kernel).
+template <class F>
+JB_DI void contact_frame_sweep(const Ctx& c, F&& on_contact) {
     const int L = KP->L;
-    bool has_free = false;
-    for (int r = 0; r < KP->nrec; ++r) {
-        const RecInt* ri = KP->rint + (r * L + c.sub);
-        if (ri->kind == REC_PAD) continue;
-        load_record_state_aos(c, ri, KP->rec_off[r], KP->q_in, KP->v_in, c.env);
-        has_free = has_free || (ri->kind == REC_FREE && ri->idx_q == 0);
-    }
     stage_from_accepted(c);
-    double zmin = D_INF;
-    bool any_contact = false;
     Xf oMc;
 #pragma unroll
     for (int k = 0; k < 9; ++k) oMc.R[k] = 0.0;
@@ -120,13 +107,36 @@ __device__ __noinline__ void place_on_ground(const Ctx c) {
         }
         for (int k = 0; k < ri->ncontact; ++k) {
             const ContactSlot* ct = KP->cslots + ((ri->contact0 + k) * L + c.sub);
-            const double z = (oM.p + rmul(oM.R, ld3(ct->placement + 9))).z;
-            zmin = (z < zmin || z != z) ? z : zmin;
-            any_contact = true;
+            on_contact(ct, oM.p + rmul(oM.R, ld3(ct->placement + 9)));
         }
         if (ri->pool >= 0) sm_store_xf(c, KP->pool_off + POOL_SIZE * ri->pool, oM);
         oMc = oM;
     }
+}
+
+// jb_start_device_on_ground: `robots.ground_base_height` on the device (the rule of BaseJiminyEnv._sample_state,
+// generic.py:1300-1335): q[2] of this env's input row is lowered or raised so that its lowest contact frame touches the
+// flat ground z = 0.  The forward kinematics runs on the row as given (before the start's quaternion normalisation), with
+// the forward sweep's joint transforms (joint_calc) and this block's model variant.  Each lane takes the min over its own
+// contact slots, then every lane reads the group's lane minima in the order 0 .. L-1, so that all of them agree bit for
+// bit.  Sub-lane 0 writes q[2] into the batch's own copy of the row (KP->q_in), which the input checks and the loads of
+// the start then read.  The min keeps a NaN, so a row that yields one still fails the checks.  Without a free-flyer at
+// q[0:7] or without a contact frame the row is left as it is.
+__device__ __noinline__ void place_on_ground(const Ctx c) {
+    const int L = KP->L;
+    bool has_free = false;
+    for (int r = 0; r < KP->nrec; ++r) {
+        const RecInt* ri = KP->rint + (r * L + c.sub);
+        if (ri->kind == REC_PAD) continue;
+        load_record_state_aos(c, ri, KP->rec_off[r], KP->q_in, KP->v_in, c.env);
+        has_free = has_free || (ri->kind == REC_FREE && ri->idx_q == 0);
+    }
+    double zmin = D_INF;
+    bool any_contact = false;
+    contact_frame_sweep(c, [&](const ContactSlot*, const V3& p) {
+        zmin = (p.z < zmin || p.z != p.z) ? p.z : zmin;
+        any_contact = true;
+    });
     double zg = D_INF;
     for (int k = 0; k < L; ++k) {
         const double z = jb_shfl(c, zmin, c.lane - c.sub + k);
@@ -907,6 +917,38 @@ __global__ void __launch_bounds__(32) env_step_kernel_model_fast(const LaunchArg
 __global__ void __launch_bounds__(32) env_step_kernel_model_ext(const LaunchArgs la) { env_step_launch<true, true, false, true>(la); }
 __global__ void __launch_bounds__(32) env_step_kernel_model(const LaunchArgs la) { env_step_launch<false, false, false, true>(la); }
 __global__ void __launch_bounds__(32) env_step_kernel_model_flex(const LaunchArgs la) { env_step_launch<false, false, true, true>(la); }
+
+// jb_contact_positions_device: world position of every contact frame of every env, out[env][contact][3], from the
+// accepted state (the SoA q of the last start / step), by the forward sweep of place_on_ground on the env's own model
+// (its variant's table, or its own table with per-env model rows).  Same lane layout and shared memory as the step
+// kernels; a kernel of its own, so that they are not touched.  Envs that are not started or carry NaN read NaN.
+__global__ void __launch_bounds__(32) contact_positions_kernel(double* __restrict__ out, int ncontacts) {
+    Ctx c;
+    c.lane = threadIdx.x & 31;
+    const int L = KP->L;
+    c.sub = c.lane % L;
+    const int env_raw = blockIdx.x * (32 / L) + c.lane / L;
+    c.valid = env_raw < KP->n_env;
+    c.env = c.valid ? env_raw : (KP->n_env - 1);
+    if (KP->pem_on) c.flags = (c.env * KP->rdbl_rows) << CTX_ROW_SHIFT;
+    else c.flags = KP->n_variants > 1 ? (KP->variant_of_block[blockIdx.x] * KP->rdbl_rows) << CTX_ROW_SHIFT : 0;
+    c.gmask = (L == 32) ? 0xffffffffu : (((1u << L) - 1u) << (c.lane - c.sub));
+    double* const o = out + static_cast<size_t>(c.env) * ncontacts * 3;
+    if (KP->status[c.env] & (JB_ENV_NOT_STARTED | JB_ENV_NAN)) {
+        if (c.valid) for (int k = c.sub; k < 3 * ncontacts; k += L) o[k] = D_NAN;
+        return;
+    }
+    for (int r = 0; r < KP->nrec; ++r) {
+        const RecInt* ri = KP->rint + (r * L + c.sub);
+        if (ri->kind != REC_PAD) load_record_state(c, ri, KP->rec_off[r], KP->q, KP->v, nullptr, KP->n_pad, c.env);
+    }
+    // a trunk contact sits in the slots of every lane of the env, with the same bits in each: every one of them writes it
+    contact_frame_sweep(c, [&](const ContactSlot* ct, const V3& p) {
+        if (!c.valid || ct->contact < 0) return;
+        double* const x = o + 3 * ct->contact;
+        x[0] = p.x; x[1] = p.y; x[2] = p.z;
+    });
+}
 
 // ---- observation exchange over peer memory: the consumer's wait (one thread)
 #ifndef JB_HOST_EMUL

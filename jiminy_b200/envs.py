@@ -17,11 +17,11 @@ the flat sensor row.
 from __future__ import annotations
 
 import functools
-from typing import Any, Dict, Optional, Tuple
+from typing import Any, Dict, Optional, Sequence, Tuple
 
 import numpy as np
 
-from . import core, model_randomisation, scenarios, sensor_randomisation
+from . import compositions, core, model_randomisation, scenarios, sensor_randomisation
 from .disturbance import from_std_ratio
 from .model import RobotTable
 
@@ -101,9 +101,11 @@ def configure_pd_blocks(env, kp, kd, joint_position_margin: float, joint_velocit
 
 
 class BatchedJiminyEnv:
+    training = True     # `training_only` termination conditions run (the PD envs take it as an argument)
+
     def __init__(self, scenario: scenarios.Scenario, device: int = 0, height_threshold_ratio: float = 0.5,
                  simulation_duration_max: float = 20.0, api_: Optional[core.Api] = None, std_ratio: Optional[dict] = None,
-                 model_bias_std: Optional[dict] = None):
+                 model_bias_std: Optional[dict] = None, reward=None, terminations: Sequence = ()):
         """`std_ratio`: the reference walker env's randomisation ratios.  None or {}: none; "disturbance": r, the walker
         disturbance forces (`jiminy_b200.disturbance`); "sensors": r, noise, bias, delay and jitter of every sensor and a
         new seed of its generators (`jiminy_b200.sensor_randomisation`); "model": r, stiffness and damping of every
@@ -111,7 +113,10 @@ class BatchedJiminyEnv:
         `model_bias_std`: the body biases of the robot options `massBodiesBiasStd`, `centerOfMassPositionBodiesBiasStd`,
         `inertiaBodiesBiasStd`, `relativePositionBodiesBiasStd` (standard deviations; None, {} or zeros: none), drawn per
         env around the nominal model (`model_randomisation.ModelBiasRandomisation`).  All are re-drawn for every env that
-        (re)starts."""
+        (re)starts.
+        `reward` / `terminations`: the reward and the extra termination conditions of the reference's composed env
+        (`jiminy_b200.compositions`; `compositions.from_config` reads them from a reference env config).  The defaults,
+        `SurviveReward` and no extra condition, are the env's plain behaviour."""
         self.sc = scenario
         self.robot: RobotTable = scenario.robot
         self.n_env, self.step_dt = scenario.n_env, scenario.step_dt
@@ -150,6 +155,10 @@ class BatchedJiminyEnv:
             self.model_bias.register(self.engine)
             self._model_bias_rng = np.random.default_rng([scenario.seed, 0xB1A5])
             self.model_bias_rows: Optional[np.ndarray] = None     # the body rows every env runs with [n_env, njoints, 13]
+        self.compositions = None
+        if reward is not None or len(terminations):
+            self.compositions = compositions.Compositions(reward, terminations, self.robot, self.n_env, self.step_dt,
+                                                          simulation_duration_max, self._height_min, self.training)
         self._started = False
 
     # ------------------------------------------------------------------ helpers
@@ -210,6 +219,7 @@ class BatchedJiminyEnv:
     # ------------------------------------------------------------------ gym API
     def reset(self, mask: Optional[np.ndarray] = None) -> Tuple[Dict[str, Any], Dict[str, Any]]:
         if mask is None or not self._started:
+            mask = None
             q0, v0 = (self.sc.q0, self.sc.v0) if not self._started else self._sample_state(self.n_env)
             self.engine.set_command(self.sc.target0)
             self._redraw_disturbance(None)
@@ -227,7 +237,31 @@ class BatchedJiminyEnv:
             self._redraw_model_bias(mask)
             self.engine.start(q0, v0, mask=mask)
             self.num_steps[mask.astype(bool)] = 0
+        self._seed_compositions(mask)
         return self._observation(), {}
+
+    def _seed_compositions(self, mask: Optional[np.ndarray]) -> None:
+        """The power stacks of the envs that have just (re)started (None: all) take the power of their start state."""
+        if self.compositions is not None:
+            self.compositions.seed(mask, self.engine.get_state()[2], self.engine.get_stepper_state()[1])
+
+    def _reward_done(self, obs, status):
+        """Reward, terminated, truncated and info after an env-step: the env's own rule, then the compositions if any."""
+        q = obs["states"]["agent"]["q"]
+        terminated, truncated = terminated_truncated(q, status, self.num_steps, self.step_dt, self.simulation_duration_max,
+                                                     self._height_min)
+        info = {"status": status}
+        if self.compositions is None:
+            return np.where(terminated, 0.0, 1.0), terminated, truncated, info      # SurviveReward
+        comp = self.compositions
+        contacts = None
+        if comp.needs_contacts:
+            models = [self.engine.model(e) for e in range(self.n_env)] if self.model_bias is not None else [self.robot] * self.n_env
+            contacts = compositions.contact_positions(models, q)
+        reward, terminated, truncated, extra = comp.evaluate(obs["t"], q, obs["states"]["agent"]["v"],
+                                                             self.engine.get_stepper_state()[1], terminated, truncated, contacts)
+        info.update(extra)
+        return reward, terminated, truncated, info
 
     def step(self, action: np.ndarray):
         """action: [n_env, nmotors] efforts (or position targets in PD mode).  Returns the gymnasium
@@ -239,11 +273,7 @@ class BatchedJiminyEnv:
         self.engine.step(self.step_dt)
         obs = self._observation()
         self.num_steps += 1
-        status = self.engine.get_status()
-        terminated, truncated = terminated_truncated(obs["states"]["agent"]["q"], status, self.num_steps, self.step_dt,
-                                                     self.simulation_duration_max, self._height_min)
-        reward = np.where(terminated, 0.0, 1.0)          # SurviveReward
-        info = {"status": status}
+        reward, terminated, truncated, info = self._reward_done(obs, self.engine.get_status())
         done = terminated | truncated
         if done.any():
             # gymnasium vector-env convention: finished envs return their first observation after the restart, the
@@ -272,6 +302,7 @@ class PDControlBatchedEnv(BatchedJiminyEnv):
                  is_instantaneous: bool = False, mahony: Optional[Tuple[float, float]] = None, training: bool = True, **kw):
         from .blocks import PDAdapter
         kp, kd = pd_gains(scenario, kp, kd)
+        self.training = training
         with without_plain_pd(scenario):          # the base class must not install the plain PD law
             super().__init__(scenario, **kw)
         deadband = configure_pd_blocks(self, kp, kd, joint_position_margin, joint_velocity_limit, joint_acceleration_limit,
@@ -298,6 +329,7 @@ class PDControlBatchedEnv(BatchedJiminyEnv):
             self.engine.start(q0, v0)
             self.num_steps[:] = 0
             self._started = True
+            self._seed_compositions(None)
             return self._observation(), {}
         return super().reset(mask)
 
@@ -309,12 +341,8 @@ class PDControlBatchedEnv(BatchedJiminyEnv):
         self.engine.step(self.step_dt)
         obs = self._observation()
         self.num_steps += 1
-        status = self.engine.get_status()
-        terminated, truncated = terminated_truncated(obs["states"]["agent"]["q"], status, self.num_steps, self.step_dt,
-                                                     self.simulation_duration_max, self._height_min)
-        reward = np.where(terminated, 0.0, 1.0)
+        reward, terminated, truncated, info = self._reward_done(obs, self.engine.get_status())
         done = terminated | truncated
-        info = {"status": status}
         if done.any():
             info["final_observation"], info["_final_observation"] = obs, done
             obs, _ = self.reset(mask=done.astype(np.uint8))

@@ -8,7 +8,10 @@ What differs from the host envs is only where the work runs:
 - the observation is read from the batch's device buffers (`jb_device_views`, `jb_state_ptrs`, `jb_device_block_views`):
   fresh tensors per observation, the same nested dict as the host envs;
 - termination, truncation and `SurviveReward` are evaluated on the device with the host envs' rule
-  (`envs.terminated_truncated`);
+  (`envs.terminated_truncated`); with `reward` / `terminations` (`jiminy_b200.compositions`), a contact-frame pass
+  (`jb_contact_positions_device`) and one composition kernel (`jb_compositions_device`) evaluate the env's rule, the
+  termination conditions and the reward tree instead, and a second launch of that kernel behind the masked restart
+  reseeds the power stacks of the restarted envs;
 - finished envs are restarted by a masked `jb_start_device` that is enqueued at EVERY step with the done mask as a device
   tensor: envs outside the mask leave at the top of the launch, so no host decision depends on device data.
 
@@ -156,6 +159,17 @@ class DeviceBatchedEnv(envs.BatchedJiminyEnv):
         nimu = self.robot.sensor_layout()["ImuSensor"][2]
         self._mahony_state = self._view(mahony, (n, nimu, 10)) if mahony else None
         self._set_action_bounds()
+        if self.compositions is not None:
+            # the spec is uploaded once; the launches' outputs live in these buffers, cloned for the caller at every step
+            comp = self.compositions
+            comp.upload(eng)
+            nc = len(self.robot.contact_frame_names)
+            self._contacts = torch.full((n, max(nc, 1), 3), float("nan"), **f64)
+            self._comp_reward = torch.zeros(n, **f64)
+            self._comp_done = torch.zeros((2, n), dtype=torch.bool, device=dev)
+            self._comp_index = torch.full((2, n), -1, dtype=torch.int32, device=dev)
+            self._comp_values = torch.full((len(comp.nodes), n), float("nan"), **f64)
+            self._all = torch.ones(n, dtype=torch.uint8, device=dev)
 
     def _set_action_bounds(self) -> None:
         f64 = dict(dtype=torch.float64, device=self.torch_device)
@@ -280,6 +294,8 @@ class DeviceBatchedEnv(envs.BatchedJiminyEnv):
         self._redraw_model_bias(done)
         self.engine.start_device(self._q_start.data_ptr(), self._v_start.data_ptr(), self._mask.data_ptr(),
                                  on_ground=self._sample_restarts)
+        if self.compositions is not None:
+            self.engine.compositions_device(self._mask.data_ptr())
         self.num_steps.masked_fill_(done, 0)
         return None if rows is None else torch.where(done, rows, torch.full_like(rows, -1))
 
@@ -297,6 +313,8 @@ class DeviceBatchedEnv(envs.BatchedJiminyEnv):
                 self._redraw_model(None)
                 self._redraw_model_bias(None)
                 self.engine.start(self.sc.q0, self.sc.v0)
+                if self.compositions is not None:
+                    self.engine.compositions_device(self._all.data_ptr())
                 self.num_steps.zero_()
                 self._started = True
             else:
@@ -328,18 +346,36 @@ class DeviceBatchedEnv(envs.BatchedJiminyEnv):
             obs = self._observation()
             self.num_steps += 1
             status = self._status.clone()
-            terminated, truncated = envs.terminated_truncated(obs["states"]["agent"]["q"], status, self.num_steps.double(),
-                                                              self.step_dt, self.simulation_duration_max, self._height_min)
-            reward = (~terminated).to(torch.float64)             # SurviveReward
+            extra: Dict[str, torch.Tensor] = {}
+            if self.compositions is None:
+                terminated, truncated = envs.terminated_truncated(obs["states"]["agent"]["q"], status, self.num_steps.double(),
+                                                                  self.step_dt, self.simulation_duration_max, self._height_min)
+                reward = (~terminated).to(torch.float64)         # SurviveReward
+            else:
+                reward, terminated, truncated, extra = self._evaluate_compositions()
             done = terminated | truncated
             rows = self._restart(done)                           # enqueued at every step: no host decision
-            info = {"status": status, "final_observation": obs, "_final_observation": done}
+            info = {"status": status, "final_observation": obs, "_final_observation": done, **extra}
             if rows is not None:
                 info["reset_rows"] = rows
             obs = self._observation()
             self._hand_over(caller, list(self._leaves(obs)) + list(self._leaves(info["final_observation"])) +
-                            [status, done, reward, terminated, truncated] + ([] if rows is None else [rows]))
+                            [status, done, reward, terminated, truncated] + list(extra.values()) + ([] if rows is None else [rows]))
         return obs, reward, terminated, truncated, info
+
+    def _evaluate_compositions(self):
+        """The contact-frame pass and the composition kernel on the batch stream: (reward, terminated, truncated, info
+        entries), fresh tensors."""
+        eng = self.engine
+        if self.compositions.needs_contacts:
+            eng.contact_positions_device(self._contacts.data_ptr())
+        eng.compositions_device(None, self.num_steps.data_ptr(), self._contacts.data_ptr(), self._comp_reward.data_ptr(),
+                                self._comp_done[0].data_ptr(), self._comp_done[1].data_ptr(), self._comp_index.data_ptr(),
+                                self._comp_values.data_ptr())
+        done, index, values = self._comp_done.clone(), self._comp_index.clone(), self._comp_values.clone()
+        extra = {"terminated": index[0], "truncated": index[1]}
+        extra.update({name: values[i] for i, name in enumerate(self.compositions.names)})
+        return self._comp_reward.clone(), done[0], done[1], extra
 
 
 class DevicePDControlBatchedEnv(DeviceBatchedEnv):
@@ -351,6 +387,7 @@ class DevicePDControlBatchedEnv(DeviceBatchedEnv):
                  safety: Optional[Dict[str, float]] = None, order: int = 1, joint_velocity_deadband: float = 0.0,
                  is_instantaneous: bool = False, mahony: Optional[Tuple[float, float]] = None, training: bool = True, **kw):
         kp, kd = envs.pd_gains(scenario, kp, kd)
+        self.training = training
         reset_states, torch_device = kw.pop("reset_states", None), kw.pop("torch_device", None)
         with envs.without_plain_pd(scenario):
             envs.BatchedJiminyEnv.__init__(self, scenario, **kw)

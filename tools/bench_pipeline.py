@@ -38,6 +38,11 @@ off and on, alternating in one process, `max(--alternate, 1)` rounds; randomisat
 ground in the start kernel (`reset_states="sample"`) against the default restart bank, alternating in one process,
 `max(--alternate, 1)` rounds; randomisation options given with it are on in both.
 
+`--compositions` times the device loop without and with a representative composition spec (`jiminy_b200.compositions`:
+roll-pitch, falling and mechanical-safety terminations, and an additive mixture of `SurviveReward` and
+`MinimizeMechanicalPowerConsumption`), alternating in one process, `max(--alternate, 1)` rounds: the cost of the
+contact-frame pass and the two composition launches per env-step.
+
     python tools/bench_pipeline.py [--robot atlas|anymal|anymal_flexible] [--loop host|device] [--alternate R]
                                    [--n-env 4096] [--steps 10] [--warmup 3] [--duration-max 0.4] [--disturbance R]
                                    [--sensors R] [--model R] [--model-bias S] [--restart bank|sample]
@@ -61,7 +66,7 @@ KEYS = [("states", "pd_controller"), ("measurements", "EncoderSensor"), ("featur
 
 def make_env(n_env: int, api_=None, robot: str = "atlas", loop: str = "host", duration_max: float = 20.0,
              disturbance: float = 0.0, sensors: float = 0.0, model: float = 0.0, restart: str = "bank",
-             model_bias: float = 0.0):
+             model_bias: float = 0.0, compositions: bool = False):
     from jiminy_b200 import envs, scenarios
     from jiminy_b200.model_randomisation import BIAS_OPTIONS
     ratio = {k: r for k, r in (("disturbance", disturbance), ("sensors", sensors), ("model", model)) if r > 0}
@@ -71,6 +76,8 @@ def make_env(n_env: int, api_=None, robot: str = "atlas", loop: str = "host", du
         if loop != "device":
             raise ValueError("--restart sample is an option of the device loop")
         kw["reset_states"] = "sample"
+    if compositions:
+        kw.update(representative_compositions(0.04 if robot == "atlas" else 0.01))
     if robot in ("anymal", "anymal_flexible"):
         from jiminy_b200.torch_envs import DeviceBatchedEnv
         return (DeviceBatchedEnv if loop == "device" else envs.BatchedJiminyEnv)(scenarios.make(robot, n_env, seed=0), **kw)
@@ -80,6 +87,16 @@ def make_env(n_env: int, api_=None, robot: str = "atlas", loop: str = "host", du
         sc, joint_position_margin=0.0, joint_velocity_limit=MOTOR_VELOCITY_MAX, joint_acceleration_limit=MOTOR_ACCELERATION_MAX,
         safety=dict(kp=1.0 / MOTOR_POSITION_MARGIN, kd=MOTOR_VELOCITY_SAFE_GAIN, soft_position_margin=0.0, soft_velocity_max=MOTOR_VELOCITY_MAX),
         order=1, mahony=(MAHONY_KP, MAHONY_KI), **kw)
+
+
+def representative_compositions(step_dt: float) -> dict:
+    """Roll-pitch, falling and mechanical-safety terminations and an additive mixture of survive and power rewards."""
+    from jiminy_b200 import compositions as CP
+    reward = CP.AdditiveMixtureReward("reward_total", [CP.SurviveReward(), CP.MinimizeMechanicalPowerConsumption(
+        cutoff=500.0, horizon=0.2)], weights=[0.5, 0.5])
+    terms = [CP.BaseRollPitchTermination(low=[-0.4, -0.4], high=[0.4, 0.4], grace_period=step_dt),
+             CP.FallingTermination(min_base_height=0.2), CP.MechanicalSafetyTermination(position_margin=0.02, velocity_max=8.0)]
+    return dict(reward=reward, terminations=terms)
 
 
 def gpu_info() -> dict:
@@ -104,10 +121,10 @@ def gpu_info() -> dict:
 
 def run(n_env: int, steps: int, warmup: int, api_=None, robot: str = "atlas", loop: str = "host",
         duration_max: float = 0.4, disturbance: float = 0.0, sensors: float = 0.0, model: float = 0.0,
-        restart: str = "bank", model_bias: float = 0.0) -> dict:
+        restart: str = "bank", model_bias: float = 0.0, compositions: bool = False) -> dict:
     import torch
     from jiminy_b200.envs import flatten_observation
-    env = make_env(n_env, api_, robot, loop, duration_max, disturbance, sensors, model, restart, model_bias)
+    env = make_env(n_env, api_, robot, loop, duration_max, disturbance, sensors, model, restart, model_bias, compositions)
     device = loop == "device"
     on_gpu = device and env.torch_device.type == "cuda"
     nm = env.robot.nmotors
@@ -181,7 +198,7 @@ def alternate(rounds: int, **kw) -> dict:
 
 def alternate_randomisation(rounds: int, ratios: dict, loops, **kw) -> dict:
     """Each loop with the randomisation of `ratios` ({"disturbance": r}, {"sensors": r}, {"model": r},
-    {"model_bias": s} or {"restart": "sample"}) off and on, `rounds` times in this process, alternating; env-steps/s and spread."""
+    {"model_bias": s}, {"restart": "sample"} or {"compositions": True}) off and on, `rounds` times in this process, alternating; env-steps/s and spread."""
     name = "_".join(ratios)
     runs = {(loop, on): [] for loop in loops for on in (False, True)}
     for _ in range(rounds):
@@ -214,10 +231,15 @@ if __name__ == "__main__":
     ap.add_argument("--model", type=float, default=0.0, metavar="R")
     ap.add_argument("--model-bias", type=float, default=0.0, metavar="S")
     ap.add_argument("--restart", choices=("bank", "sample"), default="bank")
+    ap.add_argument("--compositions", action="store_true")
     a = ap.parse_args()
     kw = dict(n_env=a.n_env, steps=a.steps, warmup=a.warmup, robot=a.robot, duration_max=a.duration_max)
     ratios = {k: r for k, r in (("disturbance", a.disturbance), ("sensors", a.sensors), ("model", a.model)) if r > 0}
-    if a.model_bias > 0:
+    if a.compositions:
+        res = alternate_randomisation(max(a.alternate, 1), {"compositions": True}, ("device",), **ratios, **kw)
+        off, on = res["device_compositions_off"], res["device_compositions_on"]
+        res["added_ms_per_env_step"] = on["ms_per_step_median"] - off["ms_per_step_median"]
+    elif a.model_bias > 0:
         if a.restart == "sample":
             kw["restart"] = "sample"
         res = alternate_randomisation(max(a.alternate, 1), {"model_bias": a.model_bias},
