@@ -2343,13 +2343,13 @@ int jb_state_ptrs(JbBatch* b, JbStateViews* host, JbStateViews* device) {
 }
 
 #if defined(JB_PROFILE_CLOCKS) && !defined(JB_HOST_EMUL)
-// development build only: read and clear the cycle counters of the full body (see jb_device.cuh)
-int jb_debug_prof(JbBatch* b, double* out16) {
+// development build only: read and clear the JB_PROF_N cycle counters (see jb_device.cuh)
+int jb_debug_prof(JbBatch* b, double* out) {
     CU(cudaSetDevice(b->device));
     CU(cudaStreamSynchronize(b->stream));
-    unsigned long long h[16];
+    unsigned long long h[JB_PROF_N];
     CU(cudaMemcpyFromSymbol(h, jb_prof, sizeof h));
-    for (int i = 0; i < 16; ++i) out16[i] = static_cast<double>(h[i]);
+    for (int i = 0; i < JB_PROF_N; ++i) out[i] = static_cast<double>(h[i]);
     std::memset(h, 0, sizeof h);
     CU(cudaMemcpyToSymbol(jb_prof, h, sizeof h));
     return JB_OK;

@@ -224,10 +224,12 @@ extern __shared__ double jb_smem[];
 // workspace slot of this block (full kernel, constraint path): the workspace is sized for the blocks that can be
 // resident at once, not for the batch, so that it stays in L2
 __shared__ int jb_cw_slot;
-// Development build only (-DJB_PROFILE_CLOCKS, tools/build_prof.sh): cycle accounting of the full body with clock64(),
-// summed over the warps of the launch (lane 0 of each warp adds its own intervals).  Never defined in the product build.
+// Development build only (-DJB_PROFILE_CLOCKS, tools/build_prof.sh): cycle accounting of the full body and of the hot-path
+// body with clock64(), summed over the warps of the launch (lane 0 of each warp adds its own intervals).  Never defined in
+// the product build.
+constexpr int JB_PROF_N = 24;
 #if defined(JB_PROFILE_CLOCKS) && !defined(JB_HOST_EMUL)
-__device__ unsigned long long jb_prof[16];
+__device__ unsigned long long jb_prof[JB_PROF_N];
 #define JB_PROF_T(var) const long long var = clock64()
 #define JB_PROF_ADD(i, t0) do { if ((threadIdx.x & 31) == 0) atomicAdd(&jb_prof[i], static_cast<unsigned long long>(clock64() - (t0))); } while (0)
 #define JB_PROF_COUNT(i, n) do { if ((threadIdx.x & 31) == 0) atomicAdd(&jb_prof[i], static_cast<unsigned long long>(n)); } while (0)
@@ -1974,6 +1976,78 @@ __device__ __noinline__ bool rhs_quadruped_crba_ext(const Ctx c, const bool up_t
 __device__ __noinline__ void stage_quadruped_crba_ext(const Ctx c, const double wq, const int kv1, const int ka1, const int kvf,
                                                       const int kaf, const double wb, int* status) {
     if (quadruped_crba<true, true>(c, false, status, wq, kv1, ka1, kvf, kaf, wb)) *status |= ENV_RETRY_FULL;
+}
+
+// FSAL repair of the quadruped hot path: the derivative at the accepted state after a controller update, from the last
+// evaluation at that same state (the FSAL stage of step_rk4_t, or an earlier repair).  Between the two only the motor
+// commands differ and the contact forces are the cached ones; the efforts enter the equations of motion linearly, so
+//     ddq_new = ddq + M^-1 [0; dtau],   dtau_j = s_j (uT_new - uT)_j
+// With the block form of M^-1 that evaluation left in shared memory -- M_ll^-1 in (DINV, U), the rows of W = M_ll^-1 M_lb
+// in FU, the legs' shares of the base Schur complement Yb in the pool entries -- that is, per leg,
+//     dy = M_ll^-1 dtau,   dg = sum_j dtau_j W_j  (summed over the lanes in a fixed order: the same bits on every lane),
+//     Yb dx = -dg,   ddq_b += dx,   ddq_l += s (dy - W dx)
+// about a tenth of the instructions of an evaluation.  uT = red uMotor (motor_effort_limited_nb, the efforts of the
+// stage form), so the old effort is read back from UMOTOR.  Returns false, touching nothing, when a joint bound is in
+// play in the env: the bound solver's correction is not linear in the efforts, and the full evaluation redoes it.
+__device__ __noinline__ bool repair_quadruped_crba(const Ctx c) {
+    using SIG = SigQuadruped;
+    constexpr int L = 4;
+    if (KP->fast_bounds) {
+        const bool mine = SMF(c, SIG::rec_off(1) + R1_BEN) != 0.0 || SMF(c, SIG::rec_off(2) + R1_BEN) != 0.0 ||
+                          SMF(c, SIG::rec_off(3) + R1_BEN) != 0.0;
+        if (jb_any(c, mine)) return false;
+    }
+    double sx[3], dtau[3], Mi[6];
+    Mot Wv[3];
+#pragma unroll
+    for (int i = 0; i < 3; ++i) {
+        const RecDbl* rd = JB_RDBL + ((i + 1) * L + c.sub);
+        const MotorConst mc = load_motor_const(rd);
+        double* const rp = jb_smem + SIG::rec_off(i + 1) * 32 + c.lane;
+        double uM, uT;
+        motor_effort_limited_nb(mc, RP(R1_CMD), RP(R1_V), uM, uT);
+        sx[i] = rd->axis[0];
+        dtau[i] = sx[i] * (uT - mc.red * RP(R1_UMOTOR));
+        RP(R1_UMOTOR) = uM;
+        Wv[i] = sm_load_mot(c, SIG::rec_off(i + 1) + R1_FU);
+        Mi[2 * i] = RP(R1_DINV); Mi[2 * i + 1] = RP(R1_U);
+    }
+    const double dy[3] = {Mi[0] * dtau[0] + Mi[1] * dtau[1] + Mi[3] * dtau[2],
+                          Mi[1] * dtau[0] + Mi[2] * dtau[1] + Mi[4] * dtau[2],
+                          Mi[3] * dtau[0] + Mi[4] * dtau[1] + Mi[5] * dtau[2]};
+    const Mot dgl = {dtau[0] * Wv[0].l + dtau[1] * Wv[1].l + dtau[2] * Wv[2].l, dtau[0] * Wv[0].a + dtau[1] * Wv[1].a + dtau[2] * Wv[2].a};
+    Mot b;
+    b.l = mk(-cq_bcast_sum4(c, dgl.l.x), -cq_bcast_sum4(c, dgl.l.y), -cq_bcast_sum4(c, dgl.l.z));
+    b.a = mk(-cq_bcast_sum4(c, dgl.a.x), -cq_bcast_sum4(c, dgl.a.y), -cq_bcast_sum4(c, dgl.a.z));
+    // Yb as the evaluation assembled it (base inertia + the lanes' pool entries in lane order)
+    SymY Yb;
+    {
+        double Kd[14];
+        load_doubles((JB_RDBL + c.sub)->placement + 12, Kd, 7);
+        inertia_to_sym(Kd[3], mk(Kd[4], Kd[5], Kd[6]), Kd + 7, Yb);
+        const double* const p0 = jb_smem + SIG::pool_off() * 32 + (c.lane - c.sub);
+#pragma unroll
+        for (int sl = 0; sl < L; ++sl) {
+#pragma unroll
+            for (int k = 0; k < 6; ++k) { Yb.A[k] += p0[k * 32 + sl]; Yb.D[k] += p0[(15 + k) * 32 + sl]; }
+#pragma unroll
+            for (int k = 0; k < 9; ++k) Yb.B[k] += p0[(6 + k) * 32 + sl];
+        }
+    }
+    Spd6 sf;
+    spd6_factor(Yb, sf);
+    const Mot dx = spd6_apply(sf, b);
+    const double dxv[6] = {dx.l.x, dx.l.y, dx.l.z, dx.a.x, dx.a.y, dx.a.z};
+    {
+        double* const rp = jb_smem + c.lane;
+        double* const ip = jb_smem + (SIG::imu_off() + 6) * 32 + c.lane;   // IMU capture: base acceleration, gravity-free frame
+#pragma unroll
+        for (int k = 0; k < 6; ++k) { RP(RF_A + k) += dxv[k]; ip[k * 32] += dxv[k]; }
+    }
+#pragma unroll
+    for (int i = 0; i < 3; ++i) SMF(c, SIG::rec_off(i + 1) + R1_A) += sx[i] * (dy[i] - (dot(Wv[i].l, dx.l) + dot(Wv[i].a, dx.a)));
+    jb_syncwarp(c);   // every lane has read the pool entries before the next evaluation rewrites them
+    return true;
 }
 
 // ------------------------------------------------------------------------------------------

@@ -641,6 +641,16 @@ __device__ __forceinline__ void env_step_body(const LaunchArgs& la, const bool o
         // Shared memory does not persist between launches: the first evaluation of this launch is a
         // full one (it rebuilds the cached contact forces, a pure function of the accepted state).
         bool need_refresh = true;
+        // fsal_linear: the last evaluation was the FSAL stage of a one-call RK4 step of the quadruped hot path, at the
+        // accepted state, and its block factors of M are still in shared memory -- the FSAL repair of a controller update
+        // is then linear (repair_quadruped_crba).  The PDController block parks its state in the U fields that hold
+        // M_ll^-1, and the force-carrying kernel can change its slots at the breakpoint: both keep the full evaluation.
+        bool fsal_linear = false;
+        bool fsal_linear_on = false;
+        if constexpr (FAST && !EXT) {
+            fsal_linear_on = KP->sig_id == SigQuadruped::ID && KP->quad_stage && KP->pdf == nullptr &&
+                             opt.ode_solver != JB_SOLVER_EULER_EXPLICIT;
+        }
 
         // stepper_->tryStep (abstract_stepper.cc:16-62) + the success / failure bookkeeping of
         // engine.cc:2132-2221.  rc: 0 success, 1 failure (adaptive step rejected), 2 error (NaN).
@@ -655,10 +665,13 @@ __device__ __forceinline__ void env_step_body(const LaunchArgs& la, const bool o
             if constexpr (!FAST || EXT) {
                 if (KP->n_proc > 0) SMF(c, proc_time_field()) = t;   // stage times of the process forces
             }
+            JB_PROF_T(t_stepper);
             if (opt.ode_solver == JB_SOLVER_EULER_EXPLICIT) { step_euler<FAST, EXT, FLEX>(c, dtLargest, &status); dtLargest = D_INF; }
             else if (FAST || opt.ode_solver == JB_SOLVER_RUNGE_KUTTA_4) { step_rk4<FAST, EXT, FLEX>(c, dtLargest, &status); dtLargest = D_INF; }
             else { if constexpr (!FAST) rc = step_dopri<FLEX>(c, &dtLargest, &status); }
+            if constexpr (FAST) { JB_PROF_ADD(16, t_stepper); JB_PROF_COUNT(21, 1); }   // hot path: stepper calls (RK4: four stage calls)
             need_refresh = false;
+            fsal_linear = fsal_linear_on;
             if constexpr (FAST) {
                 // one vote for the two rare events of a step: NaN in the new acceleration, or a joint that left its
                 // position bounds (this env is then re-done by the full kernel)
@@ -705,7 +718,9 @@ __device__ __forceinline__ void env_step_body(const LaunchArgs& la, const bool o
             if (finitePeriod && opt.controller_update_period > D_EPS) {
                 if (period_hit(t, opt.controller_update_period)) {
                     // computeCommand (engine.cc:1920-1940): zero-order hold of the action, or the PD block
+                    JB_PROF_T(t_cmd);
                     if (KP->pd_gains != nullptr || KP->pdf != nullptr) update_pd_commands(c, true);
+                    if constexpr (FAST) JB_PROF_ADD(17, t_cmd);   // hot path: controller update at a breakpoint
                     hasDynamicsChanged = true;
                 }
             }
@@ -727,12 +742,18 @@ __device__ __forceinline__ void env_step_body(const LaunchArgs& la, const bool o
                 while (tNext - t > STEPPER_MIN_TIMESTEP && !failed) {
                     if (hasDynamicsChanged) {
                         // FSAL repair: same state, cached contact forces, new command (engine.cc:2032-2037)
-                        stage_from_accepted<EXT>(c);
-                        if constexpr (!FAST || EXT) { if (KP->n_proc > 0) eval_process_forces(c, t); }
-                        if constexpr (EXT) rhs_fast_ext(c, !need_refresh, &status);
-                        else if constexpr (FAST) rhs_fast(c, !need_refresh, &status); else rhs<FLEX>(c, !need_refresh, &status);
+                        JB_PROF_T(t_repair);
+                        bool repaired = false;
+                        if constexpr (FAST && !EXT) repaired = fsal_linear && repair_quadruped_crba(c);
+                        if (!repaired) {
+                            stage_from_accepted<EXT>(c);
+                            if constexpr (!FAST || EXT) { if (KP->n_proc > 0) eval_process_forces(c, t); }
+                            if constexpr (EXT) rhs_fast_ext(c, !need_refresh, &status);
+                            else if constexpr (FAST) rhs_fast(c, !need_refresh, &status); else rhs<FLEX>(c, !need_refresh, &status);
+                        }
                         need_refresh = false;
                         hasDynamicsChanged = false;
+                        if constexpr (FAST) { JB_PROF_ADD(18, t_repair); JB_PROF_COUNT(19, 1); }   // hot path: FSAL repairs
                     }
                     if (dt < STEPPER_MIN_TIMESTEP) break;
                     double dtResidualThr = STEPPER_MIN_TIMESTEP;
@@ -771,7 +792,9 @@ __device__ __forceinline__ void env_step_body(const LaunchArgs& la, const bool o
             const double sp = opt.sensors_update_period;
             bool mustUpdateSensors = sp < D_EPS;
             if (!mustUpdateSensors) mustUpdateSensors = period_hit(t, sp);
+            JB_PROF_T(t_sensors);
             if (mustUpdateSensors) write_sensors(c, false, t);
+            if constexpr (FAST) JB_PROF_ADD(20, t_sensors);   // hot path: sensor refresh
         }
         if (!failed) t = tEnd;
     }

@@ -1,11 +1,11 @@
 #!/usr/bin/env python
 """Static SASS summary of the quadruped hot path in the step kernel (env_step_kernel_t<true>): for the RK4 step of the
-quadruped signature, the composite-rigid-body evaluation and the one-call RK4 stage, print the instruction count, the
-FP64 instruction count, basic blocks, local-memory traffic (STL / LDL), calls into the library's division / square-root
-/ trigonometric slow paths, and the spills ptxas reports.  The rows below them are the same functions of the
-force-carrying hot path (env_step_kernel_ext: the RK4 and Euler steps, the evaluation and the stage with the external-force
-slots applied).  The last rows are the same functions in the instances of batches with per-env model rows
-(env_step_kernel_model_fast, env_step_kernel_model_ext).
+quadruped signature, the composite-rigid-body evaluation, the one-call RK4 stage and the linear FSAL repair, print the
+instruction count, the FP64 instruction count, basic blocks, local-memory traffic (STL / LDL), calls into the library's
+division / square-root / trigonometric slow paths, and the spills ptxas reports.  The rows below them are the same
+functions of the force-carrying hot path (env_step_kernel_ext: the RK4 and Euler steps, the evaluation and the stage with
+the external-force slots applied).  The last rows are the same functions in the instances of batches with per-env model
+rows (env_step_kernel_model_fast, env_step_kernel_model_ext).
 
 Usage: python tools/hot_path_sass.py [--lib LIB.so [--ptxas-log LOG]]
 Without --lib the library is compiled from the tree into a temporary directory (with -Xptxas -v, for the spills).
@@ -26,6 +26,7 @@ KERNEL_MODEL_EXT = "_ZN2jb25env_step_kernel_model_extENS_10LaunchArgsE"
 FUNCS = [("step_rk4_t<FastOf<SigQuadruped>>", KERNEL, "_ZN2jb10step_rk4_tINS_6FastOfINS_13SigQuadrupedTILb0EEEEEEEvNS_3CtxEdPi"),
          ("rhs_quadruped_crba", KERNEL, "_ZN2jb18rhs_quadruped_crbaENS_3CtxEbPi"),
          ("stage_quadruped_crba", KERNEL, "_ZN2jb20stage_quadruped_crbaENS_3CtxEdiiiidPi"),
+         ("repair_quadruped_crba", KERNEL, "_ZN2jb21repair_quadruped_crbaENS_3CtxE"),
          ("step_rk4_t<FastOf<SigQuadrupedExt>>", KERNEL_EXT, "_ZN2jb10step_rk4_tINS_6FastOfINS_15SigQuadrupedExtEEEEEvNS_3CtxEdPi"),
          ("step_euler_t<FastOf<SigQuadrupedExt>>", KERNEL_EXT, "_ZN2jb12step_euler_tINS_6FastOfINS_15SigQuadrupedExtEEEEEvNS_3CtxEdPi"),
          ("rhs_quadruped_crba_ext", KERNEL_EXT, "_ZN2jb22rhs_quadruped_crba_extENS_3CtxEbPi"),
