@@ -273,6 +273,39 @@ int jb_pd_adapter_device(JbBatch* batch, const double* action_dev, double step_d
 int jb_set_mahony_filter(JbBatch* batch, double kp, double ki);
 int jb_get_mahony_filter(JbBatch* batch, double* out);
 
+/* gym_jiminy's `StackObservation` wrapper (wrappers/observation_stack.py:185-254) on the device: at every observer
+ * refresh of every env -- jb_start at t = 0, then every sensor breakpoint of jb_step, which with
+ * sensorsUpdatePeriod == controllerUpdatePeriod is the observer's refresh schedule (observe_dt = control_dt) -- the
+ * step kernel updates `num_stack` frames of the chosen leaves, oldest first, with the wrapper's rules: the latest frame
+ * always holds the current value; with skip_frames_ratio >= 0 the current value is frozen every skip_frames_ratio + 1
+ * refreshes, with -1 at every env-step breakpoint of the refresh time (step_dt of jb_step); the refresh after a freeze
+ * drops the oldest frame.  A (re)start zeroes the env's frames and applies one refresh at t = 0.  The last refresh of a
+ * jb_step sees the env's end time.  `leaves` [n_leaves] (JB_STACK_*, each at most once, in frame order): the time; a
+ * whole sensor-type block of the measured row (jb_get_sensors; field-major, jb_sensor_layout); the PDController
+ * block's action, i.e. the command buffer (target accelerations) [nmotors]; the first two rows of its state
+ * (jb_get_pd_controller_state) [2][nmotors]; the MahonyFilter quaternions, field-major [4][nimu].  A frame is the
+ * leaves one after the other.  num_stack = 0 turns stacking off.  Only between episodes (JB_ERR_BAD_CONTROL_FLOW while
+ * the batch runs); JB_ERR_NOT_IMPLEMENTED unless sensorsUpdatePeriod == controllerUpdatePeriod > 0; JB_ERR_INVALID_ARGUMENT
+ * for num_stack < 0, skip_frames_ratio < -1, no leaf, an unknown or repeated leaf, or a leaf whose sensor type or block
+ * is absent.  jb_get_obs_stack copies the frames [n_env][num_stack][frame width] to the host.  The frames are part of
+ * no checkpoint: jb_get_stepper_state / jb_set_stepper_state leave them alone. */
+#define JB_STACK_T 0
+#define JB_STACK_IMU 1
+#define JB_STACK_FORCE 2
+#define JB_STACK_ENCODER 3
+#define JB_STACK_EFFORT 4
+#define JB_STACK_CONTACT 5
+#define JB_STACK_PD_ACTION 6
+#define JB_STACK_PD_STATE 7
+#define JB_STACK_MAHONY 8
+#define JB_STACK_N_LEAF_KINDS 9
+int jb_set_obs_stack(JbBatch* batch, int32_t num_stack, int32_t skip_frames_ratio, const int32_t* leaves, int32_t n_leaves);
+int jb_get_obs_stack(JbBatch* batch, double* out);
+/* The device buffers behind jb_get_obs_stack (`stack`, NULL when stacking is off) and the command buffer jb_set_command
+ * and jb_pd_adapter_device write (`command` [n_env][nmotors]).  Any argument may be NULL.  Contents are those of the last
+ * launch that has completed on the batch stream. */
+int jb_device_obs_views(JbBatch* batch, double** stack, double** command);
+
 /* Replaces: Engine::stop (engine.cc:2419-2448): every env goes back to "not started", which is what
  * registering or removing forces requires (engine.cc:2456-2461). */
 int jb_stop(JbBatch* batch);
@@ -351,7 +384,8 @@ int jb_get_state(JbBatch* batch, double* t, double* q, double* v, double* a);
  * tPrev); command_held [n_env][nmotors].  jb_set_stepper_state overwrites whichever arrays are non-NULL (q [n_env][nq],
  * v / a [n_env][nv], iter / iter_failed [n_env]); contact forces, sensors and extra terms are rebuilt from (q, v, a)
  * by the next jb_step.  Constraint multipliers and the states of the device controller blocks are not touched (they
- * have their own getters / setters). */
+ * have their own getters / setters); neither are the stacked observation frames (jb_set_obs_stack), which have no setter:
+ * a restored batch stacks on from the frames of its last launch. */
 int jb_get_stepper_state(JbBatch* batch, double* sched, double* command_held);
 int jb_set_stepper_state(JbBatch* batch, const double* sched, const double* q, const double* v, const double* a,
                          const int64_t* iter, const int64_t* iter_failed, const double* command_held);

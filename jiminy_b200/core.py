@@ -21,6 +21,10 @@ from ._ctypes_abi import (JbModelDesc, JbOptions, JbSensorLayout, JbStateViews, 
 JB_OK = 0
 JB_ERR_INVALID_ARGUMENT, JB_ERR_BAD_CONTROL_FLOW, JB_ERR_RUNTIME, JB_ERR_NOT_IMPLEMENTED, JB_ERR_CUDA = -1, -2, -3, -4, -5
 JB_ERR_PEER_TIMEOUT = -6
+# stacked observation leaves (jb_set_obs_stack): time, a sensor-type block of the measured row, PDController action and
+# state, MahonyFilter quaternions
+STACK_T, STACK_IMU, STACK_FORCE, STACK_ENCODER, STACK_EFFORT, STACK_CONTACT = 0, 1, 2, 3, 4, 5
+STACK_PD_ACTION, STACK_PD_STATE, STACK_MAHONY = 6, 7, 8
 JB_ENV_OK, JB_ENV_NAN, JB_ENV_ITER_FAILED, JB_ENV_DT_UNDERFLOW = 0, 1, 2, 4
 JB_ENV_JOINT_LIMIT, JB_ENV_NOT_STARTED, JB_ENV_CONTACT_FORCE = 8, 16, 32
 JB_ENV_BAD_START = 256
@@ -70,7 +74,8 @@ class Api:
                "jb_set_sensor_options_env_device", "jb_set_seeds_device",
                "jb_enable_per_env_flexibility", "jb_set_flexibility_env", "jb_set_flexibility_env_device",
                "jb_get_flexibility_env", "jb_enable_per_env_model", "jb_set_model_env", "jb_set_model_env_device",
-               "jb_get_model_env", "jb_contact_positions_device", "jb_set_compositions", "jb_compositions_device")
+               "jb_get_model_env", "jb_contact_positions_device", "jb_set_compositions", "jb_compositions_device",
+               "jb_set_obs_stack", "jb_get_obs_stack", "jb_device_obs_views")
 
     def __init__(self, cdll: C.CDLL):
         self.dll = L = cdll
@@ -159,6 +164,9 @@ class Api:
         L.jb_set_compositions.argtypes = [vp, C.c_int32, C.c_int32, c_int32_p, c_double_p, C.c_int32, c_double_p, c_int32_p,
                                           c_double_p, c_double_p, C.c_int32]
         L.jb_compositions_device.argtypes = [vp] * 9
+        L.jb_set_obs_stack.argtypes = [vp, C.c_int32, C.c_int32, c_int32_p, C.c_int32]
+        L.jb_get_obs_stack.argtypes = [vp, c_double_p]
+        L.jb_device_obs_views.argtypes = [vp, C.POINTER(vp), C.POINTER(vp)]
 
     def check(self, rc: int) -> None:
         if rc != JB_OK:
@@ -407,6 +415,44 @@ class BatchedEngine:
         out = np.zeros((self.n_env, nimu, 10))
         self._api.check(self._api.dll.jb_get_mahony_filter(self._h, dptr(out)))
         return out
+
+    # ---- observation stacking (gym_jiminy's StackObservation inside the step kernel; see jiminy_b200.observation_stack)
+    def set_obs_stack(self, num_stack: int, skip_frames_ratio: int = -1, leaves: Sequence[int] = ()) -> None:
+        """Stacks `num_stack` frames of the leaves `leaves` (STACK_* codes, in frame order) at every observer refresh;
+        `num_stack=0` turns it off.  Only between episodes (BadControlFlow while envs run)."""
+        ids = np.ascontiguousarray(leaves, dtype=np.int32)
+        self._api.check(self._api.dll.jb_set_obs_stack(self._h, int(num_stack), int(skip_frames_ratio),
+                                                       ids.ctypes.data_as(c_int32_p), len(ids)))
+        # [num_stack, frame width] of the stacked frames, None when off
+        self.stack_shape = (int(num_stack), sum(self.stack_leaf_width(k) for k in ids)) if num_stack else None
+
+    def stack_leaf_width(self, leaf: int) -> int:
+        """Doubles one frame of leaf `leaf` (a STACK_* code) takes."""
+        if leaf == STACK_T:
+            return 1
+        if STACK_IMU <= leaf <= STACK_CONTACT:
+            name = ("ImuSensor", "ForceSensor", "EncoderSensor", "EffortSensor", "ContactSensor")[leaf - STACK_IMU]
+            return (6, 6, 2, 1, 3)[leaf - STACK_IMU] * self.robot.sensor_layout()[name][2]
+        if leaf == STACK_PD_ACTION:
+            return self.nm
+        if leaf == STACK_PD_STATE:
+            return 2 * self.nm
+        return 4 * self.robot.sensor_layout()["ImuSensor"][2]
+
+    def get_obs_stack(self) -> np.ndarray:
+        """The stacked frames [n_env, num_stack, frame width], oldest first (BadControlFlow when stacking is off)."""
+        if getattr(self, "stack_shape", None) is None:
+            raise BadControlFlow("observation stacking is not enabled (set_obs_stack)")
+        out = np.zeros((self.n_env,) + self.stack_shape)
+        self._api.check(self._api.dll.jb_get_obs_stack(self._h, dptr(out)))
+        return out
+
+    def device_obs_views(self) -> Tuple[int, int]:
+        """Device pointers (stacked frames [n_env, num_stack, frame width], 0 when stacking is off; command buffer
+        [n_env, nmotors])."""
+        s, c = C.c_void_p(), C.c_void_p()
+        self._api.check(self._api.dll.jb_device_obs_views(self._h, C.byref(s), C.byref(c)))
+        return s.value or 0, c.value or 0
 
     # ---- multi-GPU observation exchange over peer memory (one process per GPU)
     def peer_obs_create(self, world: int, rank: int) -> bytes:

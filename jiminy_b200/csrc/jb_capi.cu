@@ -138,6 +138,10 @@ struct JbBatch {
     int32_t *d_comp_int = nullptr, *d_comp_motor_int = nullptr, *d_comp_count = nullptr;
     double *d_comp_dbl = nullptr, *d_comp_w = nullptr, *d_comp_motor_dbl = nullptr, *d_comp_stack = nullptr;
     size_t comp_cap[7] = {};
+    // observation stacking (jb_set_obs_stack): frames, hand-off copies, refresh counters; capacities in elements
+    double *d_stk = nullptr, *d_stk_snap = nullptr;
+    int32_t *d_stk_n = nullptr, *d_stk_n_snap = nullptr;
+    size_t stk_cap[2] = {};
 };
 
 // The dynamic shared-memory opt-in is a per-function, per-device attribute: only ever raise it.
@@ -1256,6 +1260,83 @@ int jb_get_mahony_filter(JbBatch* b, double* out) {
     return JB_OK;
 }
 
+// fields of each sensor type (Imu, Force, Encoder, Effort, Contact)
+static const int kSensorFields[5] = {6, 6, 2, 1, 3};
+
+// ---- observation stacking ------------------------------------------------------------------------------------
+int jb_set_obs_stack(JbBatch* b, int32_t num_stack, int32_t skip_frames_ratio, const int32_t* leaves, int32_t n_leaves) {
+    if (!b) return fail(JB_ERR_INVALID_ARGUMENT, "null argument");
+    if (b->any_started) return fail(JB_ERR_BAD_CONTROL_FLOW, "Simulation already running. Please stop it before configuring observation stacking.");
+    if (num_stack < 0) return fail(JB_ERR_INVALID_ARGUMENT, "num_stack must be positive");
+    if (skip_frames_ratio < -1) return fail(JB_ERR_INVALID_ARGUMENT, "skip_frames_ratio must be -1 or positive");
+    if (num_stack == 0) { b->kp.stk = nullptr; return JB_OK; }
+    const JbOptions& o = b->kp.opt;
+    if (!(o.controller_update_period > 2.3e-16) || std::fabs(o.sensors_update_period - o.controller_update_period) > 1e-12)
+        return fail(JB_ERR_NOT_IMPLEMENTED, "observation stacking needs sensorsUpdatePeriod == controllerUpdatePeriod > 0 "
+                                            "(the wrapper does not support time-continuous update)");
+    if (!leaves || n_leaves < 1) return fail(JB_ERR_INVALID_ARGUMENT, "At least one observation leaf must be stacked.");
+    if (n_leaves > STACK_MAX_LEAVES) return fail(JB_ERR_INVALID_ARGUMENT, "too many stacked leaves");
+    const int counts[5] = {b->kp.nimu, b->kp.nforce, b->kp.nenc, b->kp.neff, b->kp.ncs};
+    const int offs[5] = {b->kp.lay.imu_offset, b->kp.lay.force_offset, b->kp.lay.encoder_offset, b->kp.lay.effort_offset, b->kp.lay.contact_offset};
+    const int nm = b->nmotors;
+    StackLeaf tab[STACK_MAX_LEAVES] = {};
+    bool seen[JB_STACK_N_LEAF_KINDS] = {};
+    int w = 0;
+    for (int i = 0; i < n_leaves; ++i) {
+        const int id = leaves[i];
+        if (id < 0 || id >= JB_STACK_N_LEAF_KINDS) return fail(JB_ERR_INVALID_ARGUMENT, "unknown stacked leaf " + std::to_string(id));
+        if (seen[id]) return fail(JB_ERR_INVALID_ARGUMENT, "stacked leaf " + std::to_string(id) + " given twice");
+        seen[id] = true;
+        StackLeaf& lf = tab[i];
+        if (id == JB_STACK_T) { lf.kind = STACK_T; lf.w = 1; }
+        else if (id <= JB_STACK_CONTACT) {
+            const int ty = id - JB_STACK_IMU;
+            if (!counts[ty]) return fail(JB_ERR_INVALID_ARGUMENT, "stacked leaf " + std::to_string(id) + ": the robot has no sensor of this type");
+            lf.kind = STACK_ROW; lf.src = b->d_sensors; lf.stride = b->width; lf.off = offs[ty]; lf.w = kSensorFields[ty] * counts[ty];
+        } else if (id == JB_STACK_PD_ACTION || id == JB_STACK_PD_STATE) {
+            if (!b->kp.pdf) return fail(JB_ERR_INVALID_ARGUMENT, "stacked PDController leaf: the block is not enabled (jb_set_pd_controller_full)");
+            lf.kind = STACK_ROW;
+            if (id == JB_STACK_PD_ACTION) { lf.src = b->d_cmd; lf.stride = nm; lf.w = nm; }
+            else { lf.src = b->d_pdf_state; lf.stride = 3 * nm; lf.w = 2 * nm; }
+        } else {
+            if (!b->kp.mahony) return fail(JB_ERR_INVALID_ARGUMENT, "stacked MahonyFilter leaf: the filter is not enabled (jb_set_mahony_filter)");
+            lf.kind = STACK_QUAT; lf.src = b->d_mahony; lf.stride = b->nimu; lf.w = 4 * b->nimu;
+        }
+        w += lf.w;
+    }
+    CU(cudaSetDevice(b->device));
+    const size_t n = static_cast<size_t>(b->n_env) * num_stack * w;
+    int rc = dev_reserve(b, &b->d_stk, &b->stk_cap[0], n);
+    if (!rc) rc = dev_reserve(b, &b->d_stk_snap, &b->stk_cap[1], n);
+    if (!rc && !b->d_stk_n) rc = dev_alloc(b, &b->d_stk_n, b->n_env);
+    if (!rc && !b->d_stk_n_snap) rc = dev_alloc(b, &b->d_stk_n_snap, b->n_env);
+    if (rc) return rc;
+    // frames of envs that have not started since read zero
+    CU(cudaMemsetAsync(b->d_stk, 0, sizeof(double) * n, b->stream));
+    CU(cudaStreamSynchronize(b->stream));
+    KParams& kp = b->kp;
+    kp.stk = b->d_stk; kp.stk_snap = b->d_stk_snap; kp.stk_n = b->d_stk_n; kp.stk_n_snap = b->d_stk_n_snap;
+    kp.stk_num = num_stack; kp.stk_skip = skip_frames_ratio; kp.stk_w = w; kp.stk_nleaf = n_leaves;
+    std::memcpy(kp.stk_leaf, tab, sizeof tab);
+    return JB_OK;
+}
+
+int jb_get_obs_stack(JbBatch* b, double* out) {
+    if (!b || !out) return fail(JB_ERR_INVALID_ARGUMENT, "null argument");
+    if (!b->kp.stk) return fail(JB_ERR_BAD_CONTROL_FLOW, "observation stacking is not enabled (jb_set_obs_stack)");
+    CU(cudaSetDevice(b->device));
+    CU(cudaMemcpyAsync(out, b->d_stk, sizeof(double) * b->n_env * b->kp.stk_num * b->kp.stk_w, cudaMemcpyDeviceToHost, b->stream));
+    CU(cudaStreamSynchronize(b->stream));
+    return JB_OK;
+}
+
+int jb_device_obs_views(JbBatch* b, double** stack, double** command) {
+    if (!b) return fail(JB_ERR_INVALID_ARGUMENT, "null argument");
+    if (stack) *stack = b->kp.stk;
+    if (command) *command = b->d_cmd;
+    return JB_OK;
+}
+
 int jb_get_constraints(JbBatch* b, uint8_t* joint_enabled, double* joint_lambda, uint8_t* contact_enabled, double* contact_lambda) {
     if (!b) return fail(JB_ERR_INVALID_ARGUMENT, "null argument");
     if (!b->kp.cons_on) return fail(JB_ERR_NOT_IMPLEMENTED, "no constraint state for this robot (more than 64 degrees of freedom)");
@@ -1284,7 +1365,6 @@ int jb_get_constraints(JbBatch* b, uint8_t* joint_enabled, double* joint_lambda,
 }
 
 // ---- sensor measurement pipeline ---------------------------------------------------------------------------
-static const int kSensorFields[5] = {6, 6, 2, 1, 3};
 
 int jb_set_sensor_options(JbBatch* b, int32_t type, int32_t index, const double* noise_std, const double* bias, double delay,
                           double jitter, int32_t delay_interpolation_order) {

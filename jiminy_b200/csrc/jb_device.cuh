@@ -51,6 +51,16 @@ struct SensorDesc {
     double noise_std[6], bias[6];
 };
 
+// One stacked observation leaf (jb_set_obs_stack): `w` doubles per frame, copied from the env's row of `src`
+// (src[env * stride + off + k]); STACK_T: the time of the refresh, src unused; STACK_QUAT: the quaternions of the
+// MahonyFilter state [n_env][nimu][10], field-major (k = field * nimu + imu, `stride` = nimu)
+enum : int32_t { STACK_ROW = 0, STACK_T = 1, STACK_QUAT = 2 };
+constexpr int STACK_MAX_LEAVES = 9;
+struct StackLeaf {
+    const double* src;
+    int32_t kind, stride, off, w;
+};
+
 struct KParams {
     int32_t n_env, n_pad;
     int32_t L, nrec, ntrunk, npool, ncslot, nimuslot, nfields;
@@ -206,6 +216,14 @@ struct KParams {
     double* pem_subtree;           // [n_env][njoints] subtree masses (scratch of the latch)
     double* pem_mass;              // [n_env] total mass of the env's model
     int32_t* pem_bad;              // [n_env] 1: the last device row was rejected, the env's next start refuses it
+    // observation stacking (jb_set_obs_stack, stack_observation): frames [n_env][stk_num][stk_w], oldest first, each frame
+    // the stk_nleaf leaves one after the other; null = off
+    double* stk;
+    int32_t* stk_n;                // [n_env] refreshes since the last stack update (StackObservation._n_last_stack)
+    double* stk_snap;              // [n_env][stk_num][stk_w] frames at the top of a hot-path pass (restored on hand-off)
+    int32_t* stk_n_snap;           // [n_env]
+    int32_t stk_num, stk_skip, stk_w, stk_nleaf;
+    StackLeaf stk_leaf[STACK_MAX_LEAVES];
 };
 
 // Launch parameters live in constant memory (uniform constant-bank operands in every device
@@ -3286,7 +3304,58 @@ JB_DI void mahony_update(double* ms, V3 gyro, V3 acc) {
     }
 }
 
-__device__ __noinline__ void write_sensors(const Ctx c, const bool at_start, const double t) {
+// StackObservation.refresh_observation (wrappers/observation_stack.py:221-254) at one observer refresh of the env, on the
+// measured row and the block states this refresh left.  The frames hold what the wrapper's stacked observation holds:
+// the latest frame always the current value, a shift (the refresh right after a stack update) drops the oldest frame,
+// and the frame an update freezes is the current value at that refresh.  `at_start` applies the wrapper's _setup first
+// (:207-219: zero frames, counter at skip_frames_ratio - 1).  `t_obs`: the time the observer sees (the env's end time at
+// the last refresh of a step, as the env's end-of-step refresh does); `step_dt`: the env-step, for skip_frames_ratio < 0.
+// The shift moves every column within the lane that owns it; the barriers order it against the zeroing and the leaf
+// copies, which split the columns over the lanes otherwise.
+__device__ __noinline__ void stack_observation(const Ctx c, const bool at_start, const double t_obs, const double step_dt) {
+    const int L = KP->L, S = KP->stk_num, W = KP->stk_w, skip = KP->stk_skip;
+    double* const fr = KP->stk + static_cast<size_t>(c.env) * S * W;
+    jb_syncwarp(c);   // the measured row and the Mahony state of this refresh are complete
+    if (at_start) {
+        for (int k = c.sub; k < S * W; k += L) fr[k] = 0.0;
+        jb_syncwarp(c);
+    }
+    const int n = (at_start ? skip - 1 : KP->stk_n[c.env]) + 1;
+    bool update;
+    if (skip < 0) {
+        // is_breakpoint(t, step_dt, DT_EPS) (utils/misc.py:37-49)
+        const double r = step_dt < 1e-6 ? 0.0 : fmod(t_obs, step_dt);
+        update = step_dt < 1e-6 || r < 1e-6 || step_dt - r <= 1e-6;
+    } else update = n == skip;
+    double* const last = fr + static_cast<size_t>(S - 1) * W;
+    auto write_current = [&]() {
+        int o = 0;
+        for (int i = 0; i < KP->stk_nleaf; ++i) {
+            const StackLeaf& lf = KP->stk_leaf[i];
+            for (int k = c.sub; k < lf.w; k += L) {
+                double x;
+                if (lf.kind == STACK_T) x = t_obs;
+                else if (lf.kind == STACK_QUAT) x = lf.src[(static_cast<size_t>(c.env) * lf.stride + k % lf.stride) * 10 + k / lf.stride];
+                else x = lf.src[static_cast<size_t>(c.env) * lf.stride + lf.off + k];
+                last[o + k] = x;
+            }
+            o += lf.w;
+        }
+    };
+    if (n == 0) {
+        // an update at the same refresh (skip_frames_ratio = 0) freezes the current value before the shift
+        if (update) write_current();
+        jb_syncwarp(c);
+        for (int f = 0; f + 1 < S; ++f)
+            for (int k = c.sub; k < W; k += L) fr[static_cast<size_t>(f) * W + k] = fr[static_cast<size_t>(f + 1) * W + k];
+        jb_syncwarp(c);
+    }
+    write_current();
+    jb_syncwarp(c);   // every lane has read the counter
+    if (c.sub == 0) KP->stk_n[c.env] = update ? -1 : n;
+}
+
+__device__ __noinline__ void write_sensors(const Ctx c, const bool at_start, const double t, const double t_obs, const double step_dt) {
     if (!c.valid) return;
     const int L = KP->L;
     const JbSensorLayout& lay = KP->lay;
@@ -3447,6 +3516,7 @@ __device__ __noinline__ void write_sensors(const Ctx c, const bool at_start, con
                               mk(mrow[lay.imu_offset + 3 * n + k], mrow[lay.imu_offset + 4 * n + k], mrow[lay.imu_offset + 5 * n + k]));
         }
     }
+    if (KP->stk != nullptr) stack_observation(c, at_start, t_obs, step_dt);
 }
 
 }  // namespace jb

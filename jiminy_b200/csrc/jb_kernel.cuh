@@ -238,7 +238,7 @@ __device__ __noinline__ void update_pd_commands(const Ctx c, bool running) {
 }
 
 // Copy (restore = false) or put back (restore = true) the per-env state of the device-side PDController / MahonyFilter
-// blocks.  Called by every lane of the env; the L lanes share the copy.
+// blocks, the sensor pipeline and the stacked observation.  Called by every lane of the env; the L lanes share the copy.
 __device__ __noinline__ void snapshot_blocks(const Ctx c, const int L, const bool restore) {
     if (restore) jb_syncwarp(c);   // the owner lanes' writes to the live state come first
     if (KP->pdf != nullptr) {
@@ -261,6 +261,14 @@ __device__ __noinline__ void snapshot_blocks(const Ctx c, const int L, const boo
         unsigned long long* lr = KP->sp_rng + static_cast<size_t>(c.env) * KP->sp_nsens;
         unsigned long long* sr = KP->sp_snap_rng + static_cast<size_t>(c.env) * KP->sp_nsens;
         for (int k = c.sub; k < KP->sp_nsens; k += L) { if (restore) lr[k] = sr[k]; else sr[k] = lr[k]; }
+    }
+    if (KP->stk != nullptr) {
+        // stacked observation: frames and refresh counter
+        const size_t n = static_cast<size_t>(KP->stk_num) * KP->stk_w;
+        double* live = KP->stk + static_cast<size_t>(c.env) * n;
+        double* snap = KP->stk_snap + static_cast<size_t>(c.env) * n;
+        for (size_t k = c.sub; k < n; k += L) { if (restore) live[k] = snap[k]; else snap[k] = live[k]; }
+        if (c.sub == 0) { if (restore) KP->stk_n[c.env] = KP->stk_n_snap[c.env]; else KP->stk_n_snap[c.env] = KP->stk_n[c.env]; }
     }
     jb_syncwarp(c);
 }
@@ -519,7 +527,7 @@ __device__ __forceinline__ void env_step_body(const LaunchArgs& la, const bool o
     // The stateful device blocks (PDController targets, MahonyFilter) advance inside the launch; an env handed over to
     // the full body is replayed from the top of the step, so the fast body keeps a copy to put back.
     if constexpr (FAST) {
-        if (c.valid && (KP->pdf != nullptr || KP->mahony != nullptr || KP->sp_on)) snapshot_blocks(c, L, false);
+        if (c.valid && (KP->pdf != nullptr || KP->mahony != nullptr || KP->sp_on || KP->stk != nullptr)) snapshot_blocks(c, L, false);
     }
     if constexpr (EXT) {
         if (c.valid && KP->n_prof + KP->n_proc > 0) snapshot_latched(c, L, false);
@@ -612,7 +620,7 @@ __device__ __forceinline__ void env_step_body(const LaunchArgs& la, const bool o
         bool bad = accel_has_nan(c);
         bad = jb_any(c, bad);
         if (bad) status |= JB_ENV_NAN;
-        write_sensors(c, true, 0.0);
+        write_sensors(c, true, 0.0, 0.0, 0.0);
     } else {
         t = KP->sched[SCH_T * N + col]; dt = KP->sched[SCH_DT * N + col];
         dtLargest = KP->sched[SCH_DTLARGEST * N + col]; dtLargestPrev = KP->sched[SCH_DTLARGESTPREV * N + col];
@@ -793,7 +801,8 @@ __device__ __forceinline__ void env_step_body(const LaunchArgs& la, const bool o
             bool mustUpdateSensors = sp < D_EPS;
             if (!mustUpdateSensors) mustUpdateSensors = period_hit(t, sp);
             JB_PROF_T(t_sensors);
-            if (mustUpdateSensors) write_sensors(c, false, t);
+            // (the observer of the env-step's last refresh sees the env's end time, as after the step)
+            if (mustUpdateSensors) write_sensors(c, false, t, tEnd - t >= STEPPER_MIN_TIMESTEP ? t : tEnd, stepSize);
             if constexpr (FAST) JB_PROF_ADD(20, t_sensors);   // hot path: sensor refresh
         }
         if (!failed) t = tEnd;
@@ -802,7 +811,7 @@ __device__ __forceinline__ void env_step_body(const LaunchArgs& la, const bool o
     // ---------------- store
     if constexpr (FAST) {
         if (jb_any(c, (status & ENV_RETRY_FULL) != 0)) {   // nothing of this pass is kept: the full body redoes the env
-            if (c.valid && (KP->pdf != nullptr || KP->mahony != nullptr || KP->sp_on)) snapshot_blocks(c, L, true);
+            if (c.valid && (KP->pdf != nullptr || KP->mahony != nullptr || KP->sp_on || KP->stk != nullptr)) snapshot_blocks(c, L, true);
             if constexpr (EXT) { if (c.valid && KP->n_prof + KP->n_proc > 0) snapshot_latched(c, L, true); }
             if (c.sub == 0) *needs_full = 1;
             return;

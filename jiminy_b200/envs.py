@@ -22,6 +22,7 @@ from typing import Any, Dict, Optional, Sequence, Tuple
 import numpy as np
 
 from . import compositions, core, model_randomisation, scenarios, sensor_randomisation
+from .observation_stack import StackObservation
 from .disturbance import from_std_ratio
 from .model import RobotTable
 
@@ -105,7 +106,8 @@ class BatchedJiminyEnv:
 
     def __init__(self, scenario: scenarios.Scenario, device: int = 0, height_threshold_ratio: float = 0.5,
                  simulation_duration_max: float = 20.0, api_: Optional[core.Api] = None, std_ratio: Optional[dict] = None,
-                 model_bias_std: Optional[dict] = None, reward=None, terminations: Sequence = ()):
+                 model_bias_std: Optional[dict] = None, reward=None, terminations: Sequence = (),
+                 stack: Optional[StackObservation] = None):
         """`std_ratio`: the reference walker env's randomisation ratios.  None or {}: none; "disturbance": r, the walker
         disturbance forces (`jiminy_b200.disturbance`); "sensors": r, noise, bias, delay and jitter of every sensor and a
         new seed of its generators (`jiminy_b200.sensor_randomisation`); "model": r, stiffness and damping of every
@@ -116,7 +118,10 @@ class BatchedJiminyEnv:
         (re)starts.
         `reward` / `terminations`: the reward and the extra termination conditions of the reference's composed env
         (`jiminy_b200.compositions`; `compositions.from_config` reads them from a reference env config).  The defaults,
-        `SurviveReward` and no extra condition, are the env's plain behaviour."""
+        `SurviveReward` and no extra condition, are the env's plain behaviour.
+        `stack`: gym_jiminy's `StackObservation` wrapper (`jiminy_b200.observation_stack`; `observation_stack.from_config`
+        reads it from a reference pipeline config): each stacked leaf of the observation becomes its frames
+        `[n_env, num_stack, ...]`, updated by the step kernel at every observer refresh.  None: no stacking."""
         self.sc = scenario
         self.robot: RobotTable = scenario.robot
         self.n_env, self.step_dt = scenario.n_env, scenario.step_dt
@@ -160,9 +165,46 @@ class BatchedJiminyEnv:
             self.compositions = compositions.Compositions(reward, terminations, self.robot, self.n_env, self.step_dt,
                                                           simulation_duration_max, self._height_min, self.training)
         self._started = False
+        self._setup_stack(stack)
 
     # ------------------------------------------------------------------ helpers
+    def _obs_shapes(self) -> Dict[str, Any]:
+        """The observation tree with the per-env shape of every leaf, in the order of `_observation`."""
+        meas = {name: (nf, self._layout[name][2]) for name, nf in SENSOR_FIELDS.items() if self._layout[name][2]}
+        return {"t": (), "states": {"agent": {"q": (self.robot.nq,), "v": (self.robot.nv,)}}, "measurements": meas}
+
+    def _setup_stack(self, stack: Optional[StackObservation]) -> None:
+        """Resolves the stacked leaves against the observation tree and configures the step kernel's stacking;
+        `_stack_leaves` holds (path, first column, width, per-env shape) of each in the frame."""
+        self.stack, self._stack_leaves = stack, []
+        if stack is None:
+            return
+        shapes = self._obs_shapes()
+        leaves = stack.resolve(shapes)
+        self.engine.set_obs_stack(stack.num_stack, stack.skip_frames_ratio, [code for _, code in leaves])
+        col = 0
+        for path, code in leaves:
+            shape = shapes
+            for k in path:
+                shape = shape[k]
+            width = self.engine.stack_leaf_width(code)
+            self._stack_leaves.append((path, col, width, tuple(shape)))
+            col += width
+
+    def _apply_stack(self, obs: Dict[str, Any], frames) -> Dict[str, Any]:
+        """Replaces each stacked leaf of `obs` by its frames, from `frames` [n_env, num_stack, frame width] (numpy or torch)."""
+        for path, col, width, shape in self._stack_leaves:
+            node = obs
+            for k in path[:-1]:
+                node = node[k]
+            node[path[-1]] = frames[:, :, col:col + width].reshape((self.n_env, self.stack.num_stack) + shape)
+        return obs
+
     def _observation(self) -> Dict[str, Any]:
+        obs = self._plain_observation()
+        return self._apply_stack(obs, self.engine.get_obs_stack()) if self._stack_leaves else obs
+
+    def _plain_observation(self) -> Dict[str, Any]:
         t, q, v, _ = self.engine.get_state()
         sens = np.empty_like(self._sens)      # a fresh matrix per observation: earlier observations stay valid
         self.engine.get_sensors(sens)
@@ -286,6 +328,17 @@ class BatchedJiminyEnv:
         self.engine.close()
 
 
+def pd_obs_shapes(env, shapes: Dict[str, Any]) -> Dict[str, Any]:
+    """The leaves a PD env adds to the observation tree of `_obs_shapes`, in the order of its `_observation`."""
+    nm = env.robot.nmotors
+    shapes["states"]["pd_controller"] = (2, nm)
+    if env._mahony:
+        shapes["features"] = {"mahony_filter": (4, env.robot.sensor_layout()["ImuSensor"][2])}
+    if env.augment_observation:
+        shapes["actions"] = {"pd_controller": (nm,)}
+    return shapes
+
+
 class PDControlBatchedEnv(BatchedJiminyEnv):
     """Batched counterpart of the `*PDControlJiminyEnv` pipelines that `build_pipeline` assembles in the reference
     (e.g. `AtlasPDControlJiminyEnv`, python/gym_jiminy/envs/gym_jiminy/envs/atlas.py:239-295):
@@ -294,27 +347,37 @@ class PDControlBatchedEnv(BatchedJiminyEnv):
     host once per env-step (jiminy_b200/blocks.py).  Constructor arguments and the bounds derived from them follow the
     reference's block constructors (blocks/proportional_derivative_controller.py:301-450, :560-640;
     blocks/motor_safety_limit.py:112-175).  The action is the adapter's: target motor velocities (order 1) or
-    positions (order 0) at the end of the step, within the controller's command-state bounds."""
+    positions (order 0) at the end of the step, within the controller's command-state bounds.
+    `augment_observation=True` adds the controller's action, the target accelerations of the env-step
+    (`obs["actions"]["pd_controller"]`), as the reference's `ControlledJiminyEnv` does (bases/pipeline.py:1134-1141)."""
 
     def __init__(self, scenario: scenarios.Scenario, *, kp=None, kd=None, joint_position_margin: float = 0.0,
                  joint_velocity_limit: float = float("inf"), joint_acceleration_limit: Optional[float] = None,
                  safety: Optional[Dict[str, float]] = None, order: int = 1, joint_velocity_deadband: float = 0.0,
-                 is_instantaneous: bool = False, mahony: Optional[Tuple[float, float]] = None, training: bool = True, **kw):
+                 is_instantaneous: bool = False, mahony: Optional[Tuple[float, float]] = None, training: bool = True,
+                 augment_observation: bool = False, stack: Optional[StackObservation] = None, **kw):
         from .blocks import PDAdapter
         kp, kd = pd_gains(scenario, kp, kd)
         self.training = training
+        self.augment_observation = augment_observation
         with without_plain_pd(scenario):          # the base class must not install the plain PD law
             super().__init__(scenario, **kw)
         deadband = configure_pd_blocks(self, kp, kd, joint_position_margin, joint_velocity_limit, joint_acceleration_limit,
                                        safety, order, joint_velocity_deadband, mahony, training)
+        self._setup_stack(stack)
         self.adapter = PDAdapter(self.engine, self.command_state_lower, self.command_state_upper, order=order,
                                  is_instantaneous=is_instantaneous, velocity_deadband=deadband, step_dt=self.step_dt)
 
-    def _observation(self) -> Dict[str, Any]:
-        obs = super()._observation()
+    def _obs_shapes(self) -> Dict[str, Any]:
+        return pd_obs_shapes(self, super()._obs_shapes())
+
+    def _plain_observation(self) -> Dict[str, Any]:
+        obs = super()._plain_observation()
         obs["states"]["pd_controller"] = self.engine.get_pd_controller_state()[:, :2]       # PDController.get_state (:488-489)
         if self._mahony:
             obs["features"] = {"mahony_filter": np.swapaxes(self.engine.get_mahony_filter()[:, :, :4], 1, 2)}   # [n, 4, n_imu]
+        if self.augment_observation:
+            obs["actions"] = {"pd_controller": self.engine.get_efforts()[2]}      # the block's action (pipeline.py:1134-1141)
         return obs
 
     def reset(self, mask: Optional[np.ndarray] = None):

@@ -5,8 +5,9 @@ host.
 What differs from the host envs is only where the work runs:
 - the action is clipped on the device and handed to the step kernel (`jb_set_command_device`) or, in PD mode, to the
   device `PDAdapter` kernel (`jb_pd_adapter_device`), which writes the target accelerations in place;
-- the observation is read from the batch's device buffers (`jb_device_views`, `jb_state_ptrs`, `jb_device_block_views`):
-  fresh tensors per observation, the same nested dict as the host envs;
+- the observation is read from the batch's device buffers (`jb_device_views`, `jb_state_ptrs`, `jb_device_block_views`,
+  `jb_device_obs_views` for the stacked frames of `stack=` and the PD action of `augment_observation=True`): fresh tensors
+  per observation, the same nested dict as the host envs;
 - termination, truncation and `SurviveReward` are evaluated on the device with the host envs' rule
   (`envs.terminated_truncated`); with `reward` / `terminations` (`jiminy_b200.compositions`), a contact-frame pass
   (`jb_contact_positions_device`) and one composition kernel (`jb_compositions_device`) evaluate the env's rule, the
@@ -158,6 +159,9 @@ class DeviceBatchedEnv(envs.BatchedJiminyEnv):
         self._pd_state = self._view(pd_state, (n, 3, self.robot.nmotors)) if pd_state else None
         nimu = self.robot.sensor_layout()["ImuSensor"][2]
         self._mahony_state = self._view(mahony, (n, nimu, 10)) if mahony else None
+        stack, command = eng.device_obs_views()
+        self._command = self._view(command, (n, self.robot.nmotors)) if self.robot.nmotors else None
+        self._stack_frames = self._view(stack, (n,) + eng.stack_shape) if self._stack_leaves else None
         self._set_action_bounds()
         if self.compositions is not None:
             # the spec is uploaded once; the launches' outputs live in these buffers, cloned for the caller at every step
@@ -203,6 +207,10 @@ class DeviceBatchedEnv(envs.BatchedJiminyEnv):
 
     # ------------------------------------------------------------------ observation
     def _observation(self) -> Dict[str, Any]:
+        obs = self._plain_observation()
+        return self._apply_stack(obs, self._stack_frames.clone()) if self._stack_leaves else obs
+
+    def _plain_observation(self) -> Dict[str, Any]:
         nq = self.robot.nq
         qv, sens = self._qv.clone(), self._sensors.clone()      # fresh tensors: earlier observations stay valid
         meas = {}
@@ -380,27 +388,36 @@ class DeviceBatchedEnv(envs.BatchedJiminyEnv):
 
 class DevicePDControlBatchedEnv(DeviceBatchedEnv):
     """`PDControlBatchedEnv` (MotorSafetyLimit -> PDController -> PDAdapter -> MahonyFilter) with the adapter on the device
-    as well: same constructor arguments and bounds (`envs.configure_pd_blocks`), plus those of `DeviceBatchedEnv`."""
+    as well: same constructor arguments and bounds (`envs.configure_pd_blocks`), `augment_observation` and `stack`
+    included, plus those of `DeviceBatchedEnv`."""
 
     def __init__(self, scenario: scenarios.Scenario, *, kp=None, kd=None, joint_position_margin: float = 0.0,
                  joint_velocity_limit: float = float("inf"), joint_acceleration_limit: Optional[float] = None,
                  safety: Optional[Dict[str, float]] = None, order: int = 1, joint_velocity_deadband: float = 0.0,
-                 is_instantaneous: bool = False, mahony: Optional[Tuple[float, float]] = None, training: bool = True, **kw):
+                 is_instantaneous: bool = False, mahony: Optional[Tuple[float, float]] = None, training: bool = True,
+                 augment_observation: bool = False, stack=None, **kw):
         kp, kd = envs.pd_gains(scenario, kp, kd)
         self.training = training
+        self.augment_observation = augment_observation
         reset_states, torch_device = kw.pop("reset_states", None), kw.pop("torch_device", None)
         with envs.without_plain_pd(scenario):
             envs.BatchedJiminyEnv.__init__(self, scenario, **kw)
         deadband = envs.configure_pd_blocks(self, kp, kd, joint_position_margin, joint_velocity_limit, joint_acceleration_limit,
                                             safety, order, joint_velocity_deadband, mahony, training)
         self.engine.set_pd_adapter(order, is_instantaneous, deadband)
+        self._setup_stack(stack)
         self._init_device(reset_states, torch_device, kw.get("api_"))
 
-    def _observation(self) -> Dict[str, Any]:
-        obs = super()._observation()
+    def _obs_shapes(self) -> Dict[str, Any]:
+        return envs.pd_obs_shapes(self, super()._obs_shapes())
+
+    def _plain_observation(self) -> Dict[str, Any]:
+        obs = super()._plain_observation()
         obs["states"]["pd_controller"] = self._pd_state[:, :2].clone()      # PDController.get_state (:488-489)
         if self._mahony:
             obs["features"] = {"mahony_filter": self._mahony_state[:, :, :4].transpose(1, 2).clone()}   # [n, 4, n_imu]
+        if self.augment_observation:
+            obs["actions"] = {"pd_controller": self._command.clone()}         # the block's action (pipeline.py:1134-1141)
         return obs
 
     def _apply_action(self, action: torch.Tensor) -> None:

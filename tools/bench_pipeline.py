@@ -43,9 +43,15 @@ roll-pitch, falling and mechanical-safety terminations, and an additive mixture 
 `MinimizeMechanicalPowerConsumption`), alternating in one process, `max(--alternate, 1)` rounds: the cost of the
 contact-frame pass and the two composition launches per env-step.
 
+`--stack NUM,SKIP` times the device loop without and with observation stacking (`jiminy_b200.observation_stack`,
+num_stack NUM, skip_frames_ratio SKIP), alternating in one process, `max(--alternate, 1)` rounds.  The stacked leaves are
+`t`, `measurements.ImuSensor` and 12 doubles of motor data, 19 doubles per frame: `measurements.EffortSensor` on the
+plain-PD ANYmal and anymal_flexible envs, the PDController's action (`augment_observation=True`) on Atlas.
+
     python tools/bench_pipeline.py [--robot atlas|anymal|anymal_flexible] [--loop host|device] [--alternate R]
                                    [--n-env 4096] [--steps 10] [--warmup 3] [--duration-max 0.4] [--disturbance R]
-                                   [--sensors R] [--model R] [--model-bias S] [--restart bank|sample]
+                                   [--sensors R] [--model R] [--model-bias S] [--restart bank|sample] [--compositions]
+                                   [--stack NUM,SKIP]
 """
 import argparse
 import json
@@ -66,8 +72,9 @@ KEYS = [("states", "pd_controller"), ("measurements", "EncoderSensor"), ("featur
 
 def make_env(n_env: int, api_=None, robot: str = "atlas", loop: str = "host", duration_max: float = 20.0,
              disturbance: float = 0.0, sensors: float = 0.0, model: float = 0.0, restart: str = "bank",
-             model_bias: float = 0.0, compositions: bool = False):
+             model_bias: float = 0.0, compositions: bool = False, stack=None):
     from jiminy_b200 import envs, scenarios
+    from jiminy_b200.observation_stack import StackObservation
     from jiminy_b200.model_randomisation import BIAS_OPTIONS
     ratio = {k: r for k, r in (("disturbance", disturbance), ("sensors", sensors), ("model", model)) if r > 0}
     kw = dict(simulation_duration_max=duration_max, api_=api_, std_ratio=ratio or None,
@@ -78,6 +85,11 @@ def make_env(n_env: int, api_=None, robot: str = "atlas", loop: str = "host", du
         kw["reset_states"] = "sample"
     if compositions:
         kw.update(representative_compositions(0.04 if robot == "atlas" else 0.01))
+    if stack is not None:
+        motors = ("measurements", "EffortSensor") if robot != "atlas" else ("actions",)
+        kw["stack"] = StackObservation(stack[0], [("t",), ("measurements", "ImuSensor"), motors], stack[1])
+        if robot == "atlas":
+            kw["augment_observation"] = True
     if robot in ("anymal", "anymal_flexible"):
         from jiminy_b200.torch_envs import DeviceBatchedEnv
         return (DeviceBatchedEnv if loop == "device" else envs.BatchedJiminyEnv)(scenarios.make(robot, n_env, seed=0), **kw)
@@ -121,10 +133,10 @@ def gpu_info() -> dict:
 
 def run(n_env: int, steps: int, warmup: int, api_=None, robot: str = "atlas", loop: str = "host",
         duration_max: float = 0.4, disturbance: float = 0.0, sensors: float = 0.0, model: float = 0.0,
-        restart: str = "bank", model_bias: float = 0.0, compositions: bool = False) -> dict:
+        restart: str = "bank", model_bias: float = 0.0, compositions: bool = False, stack=None) -> dict:
     import torch
     from jiminy_b200.envs import flatten_observation
-    env = make_env(n_env, api_, robot, loop, duration_max, disturbance, sensors, model, restart, model_bias, compositions)
+    env = make_env(n_env, api_, robot, loop, duration_max, disturbance, sensors, model, restart, model_bias, compositions, stack)
     device = loop == "device"
     on_gpu = device and env.torch_device.type == "cuda"
     nm = env.robot.nmotors
@@ -167,7 +179,7 @@ def run(n_env: int, steps: int, warmup: int, api_=None, robot: str = "atlas", lo
             f"contacts, euler_explicit 5 ms" if robot == "atlas" else
             f"{robot} PD standing (plain PD law), spring-damper contacts, runge_kutta_4 1 ms, per-step position targets")
     out = {"metric": "env_steps_per_sec", "unit": "env-steps/s", "value": n_env * steps / dt, "ms_per_step": 1e3 * dt / steps,
-           "loop": loop, "restart": restart, "robot": robot, "disturbance": disturbance, "sensors": sensors, "model": model, "model_bias": model_bias, "n_env": n_env, "steps": steps, "warmup": warmup,
+           "loop": loop, "restart": restart, "stack": stack, "robot": robot, "disturbance": disturbance, "sensors": sensors, "model": model, "model_bias": model_bias, "n_env": n_env, "steps": steps, "warmup": warmup,
            "timing": "host clock around env.step + flatten_observation, ending in a device synchronise",
            "config": {"workload": f"{desc}, {n_env} envs, step_dt {env.step_dt}, simulation_duration_max {duration_max}",
                       "env": type(env).__name__, "lane_plan": env.engine.describe(), "observation_width": int(flat.shape[1])},
@@ -198,7 +210,7 @@ def alternate(rounds: int, **kw) -> dict:
 
 def alternate_randomisation(rounds: int, ratios: dict, loops, **kw) -> dict:
     """Each loop with the randomisation of `ratios` ({"disturbance": r}, {"sensors": r}, {"model": r},
-    {"model_bias": s}, {"restart": "sample"} or {"compositions": True}) off and on, `rounds` times in this process, alternating; env-steps/s and spread."""
+    {"model_bias": s}, {"restart": "sample"}, {"compositions": True} or {"stack": (num, skip)}) off and on, `rounds` times in this process, alternating; env-steps/s and spread."""
     name = "_".join(ratios)
     runs = {(loop, on): [] for loop in loops for on in (False, True)}
     for _ in range(rounds):
@@ -232,10 +244,16 @@ if __name__ == "__main__":
     ap.add_argument("--model-bias", type=float, default=0.0, metavar="S")
     ap.add_argument("--restart", choices=("bank", "sample"), default="bank")
     ap.add_argument("--compositions", action="store_true")
+    ap.add_argument("--stack", type=str, default=None, metavar="NUM,SKIP")
     a = ap.parse_args()
     kw = dict(n_env=a.n_env, steps=a.steps, warmup=a.warmup, robot=a.robot, duration_max=a.duration_max)
     ratios = {k: r for k, r in (("disturbance", a.disturbance), ("sensors", a.sensors), ("model", a.model)) if r > 0}
-    if a.compositions:
+    if a.stack is not None:
+        num, skip = (int(x) for x in a.stack.split(","))
+        res = alternate_randomisation(max(a.alternate, 1), {"stack": (num, skip)}, ("device",), **ratios, **kw)
+        off, on = res["device_stack_off"], res["device_stack_on"]
+        res["added_ms_per_env_step"] = on["ms_per_step_median"] - off["ms_per_step_median"]
+    elif a.compositions:
         res = alternate_randomisation(max(a.alternate, 1), {"compositions": True}, ("device",), **ratios, **kw)
         off, on = res["device_compositions_off"], res["device_compositions_on"]
         res["added_ms_per_env_step"] = on["ms_per_step_median"] - off["ms_per_step_median"]
