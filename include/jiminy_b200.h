@@ -273,6 +273,31 @@ int jb_pd_adapter_device(JbBatch* batch, const double* action_dev, double step_d
 int jb_set_mahony_filter(JbBatch* batch, double kp, double ki);
 int jb_get_mahony_filter(JbBatch* batch, double* out);
 
+/* The MahonyFilter with the reference's full option set (jb_set_mahony_filter is this call with exact_init = 1,
+ * ignore_twist = 0, compute_rpy = 0, and the same state).  exact_init = 0: at a (re)start the estimate is the swing of
+ * the measured accelerometer (`swing_from_vector`, utils/math.py:1066-1137), or the true orientation when every
+ * component of the measured acceleration is below 0.1 g (free fall); the start applies no iteration and no twist
+ * removal.  ignore_twist: `remove_twist_from_quat` (utils/math.py:1203-1246) after every iteration.  compute_rpy:
+ * `quat_to_rpy` (utils/math.py:159-197) after the start and after every iteration. */
+int jb_set_mahony_filter_full(JbBatch* batch, double kp, double ki, int32_t exact_init, int32_t ignore_twist, int32_t compute_rpy);
+
+/* gym_jiminy's `BodyObserver` (blocks/body_orientation_observer.py:26-266) on the device, refreshed right after the
+ * MahonyFilter at the same times (jb_start at t = 0, then every sensor refresh): the parent body's orientation
+ * quat_multiply(q_imu, q_rel, is_right_conjugate=True) and angular velocity q_rel.apply(omega_imu), q_rel the IMU frame's
+ * placement rotation in its parent body; twist_time_constant NaN (None) keeps the filter's twist, 0 removes it, > 0
+ * removes it and re-estimates it with `update_twist`'s leaky integrator (dt = sensorsUpdatePeriod, zero twist at every
+ * (re)start, one update at the start refresh as at the reference's reset); compute_rpy adds `quat_to_rpy`.  enable = 0
+ * turns it off.  Only between episodes (JB_ERR_BAD_CONTROL_FLOW while the batch runs); JB_ERR_INVALID_ARGUMENT without
+ * the MahonyFilter or for a negative or infinite time constant.  Turning the MahonyFilter off turns it off too.
+ * jb_get_observers copies [n_env][nimu][14] to the host: the filter's roll-pitch-yaw (3), the body's quaternion (4),
+ * roll-pitch-yaw (3), angular velocity (3) and twist angle (1); fields of an option that is off hold no meaning.
+ * JB_ERR_BAD_CONTROL_FLOW when the filter runs its default path only (no record). */
+int jb_set_body_observer(JbBatch* batch, int32_t enable, double twist_time_constant, int32_t compute_rpy);
+int jb_get_observers(JbBatch* batch, double* out);
+/* The device buffer behind jb_get_observers (NULL when there is none); contents are those of the last launch that has
+ * completed on the batch stream. */
+int jb_device_observer_views(JbBatch* batch, double** observers);
+
 /* gym_jiminy's `StackObservation` wrapper (wrappers/observation_stack.py:185-254) on the device: at every observer
  * refresh of every env -- jb_start at t = 0, then every sensor breakpoint of jb_step, which with
  * sensorsUpdatePeriod == controllerUpdatePeriod is the observer's refresh schedule (observe_dt = control_dt) -- the
@@ -283,7 +308,9 @@ int jb_get_mahony_filter(JbBatch* batch, double* out);
  * jb_step sees the env's end time.  `leaves` [n_leaves] (JB_STACK_*, each at most once, in frame order): the time; a
  * whole sensor-type block of the measured row (jb_get_sensors; field-major, jb_sensor_layout); the PDController
  * block's action, i.e. the command buffer (target accelerations) [nmotors]; the first two rows of its state
- * (jb_get_pd_controller_state) [2][nmotors]; the MahonyFilter quaternions, field-major [4][nimu].  A frame is the
+ * (jb_get_pd_controller_state) [2][nmotors]; the MahonyFilter quaternions, field-major [4][nimu]; its angular velocity
+ * [3][nimu], roll-pitch-yaw [3][nimu] (compute_rpy) and gyro bias [3][nimu]; the BodyObserver's quaternion [4][nimu],
+ * roll-pitch-yaw [3][nimu] (compute_rpy) and angular velocity [3][nimu].  A frame is the
  * leaves one after the other.  num_stack = 0 turns stacking off.  Only between episodes (JB_ERR_BAD_CONTROL_FLOW while
  * the batch runs); JB_ERR_NOT_IMPLEMENTED unless sensorsUpdatePeriod == controllerUpdatePeriod > 0; JB_ERR_INVALID_ARGUMENT
  * for num_stack < 0, skip_frames_ratio < -1, no leaf, an unknown or repeated leaf, or a leaf whose sensor type or block
@@ -298,7 +325,13 @@ int jb_get_mahony_filter(JbBatch* batch, double* out);
 #define JB_STACK_PD_ACTION 6
 #define JB_STACK_PD_STATE 7
 #define JB_STACK_MAHONY 8
-#define JB_STACK_N_LEAF_KINDS 9
+#define JB_STACK_MAHONY_OMEGA 9
+#define JB_STACK_MAHONY_RPY 10
+#define JB_STACK_MAHONY_BIAS 11
+#define JB_STACK_BODY_QUAT 12
+#define JB_STACK_BODY_RPY 13
+#define JB_STACK_BODY_OMEGA 14
+#define JB_STACK_N_LEAF_KINDS 15
 int jb_set_obs_stack(JbBatch* batch, int32_t num_stack, int32_t skip_frames_ratio, const int32_t* leaves, int32_t n_leaves);
 int jb_get_obs_stack(JbBatch* batch, double* out);
 /* The device buffers behind jb_get_obs_stack (`stack`, NULL when stacking is off) and the command buffer jb_set_command

@@ -22,9 +22,14 @@ JB_OK = 0
 JB_ERR_INVALID_ARGUMENT, JB_ERR_BAD_CONTROL_FLOW, JB_ERR_RUNTIME, JB_ERR_NOT_IMPLEMENTED, JB_ERR_CUDA = -1, -2, -3, -4, -5
 JB_ERR_PEER_TIMEOUT = -6
 # stacked observation leaves (jb_set_obs_stack): time, a sensor-type block of the measured row, PDController action and
-# state, MahonyFilter quaternions
+# state, MahonyFilter quaternions, angular velocity, roll-pitch-yaw and gyro bias, BodyObserver quaternions,
+# roll-pitch-yaw and angular velocity
 STACK_T, STACK_IMU, STACK_FORCE, STACK_ENCODER, STACK_EFFORT, STACK_CONTACT = 0, 1, 2, 3, 4, 5
 STACK_PD_ACTION, STACK_PD_STATE, STACK_MAHONY = 6, 7, 8
+STACK_MAHONY_OMEGA, STACK_MAHONY_RPY, STACK_MAHONY_BIAS, STACK_BODY_QUAT, STACK_BODY_RPY, STACK_BODY_OMEGA = 9, 10, 11, 12, 13, 14
+# fields of the per-IMU observer record (jb_get_observers): MahonyFilter roll-pitch-yaw, BodyObserver quaternion,
+# roll-pitch-yaw, angular velocity, twist angle
+OBSV_MAHONY_RPY, OBSV_BODY_QUAT, OBSV_BODY_RPY, OBSV_BODY_OMEGA, OBSV_TWIST, OBSV_N = 0, 3, 7, 10, 13, 14
 JB_ENV_OK, JB_ENV_NAN, JB_ENV_ITER_FAILED, JB_ENV_DT_UNDERFLOW = 0, 1, 2, 4
 JB_ENV_JOINT_LIMIT, JB_ENV_NOT_STARTED, JB_ENV_CONTACT_FORCE = 8, 16, 32
 JB_ENV_BAD_START = 256
@@ -75,7 +80,8 @@ class Api:
                "jb_enable_per_env_flexibility", "jb_set_flexibility_env", "jb_set_flexibility_env_device",
                "jb_get_flexibility_env", "jb_enable_per_env_model", "jb_set_model_env", "jb_set_model_env_device",
                "jb_get_model_env", "jb_contact_positions_device", "jb_set_compositions", "jb_compositions_device",
-               "jb_set_obs_stack", "jb_get_obs_stack", "jb_device_obs_views")
+               "jb_set_obs_stack", "jb_get_obs_stack", "jb_device_obs_views",
+               "jb_set_mahony_filter_full", "jb_set_body_observer", "jb_get_observers", "jb_device_observer_views")
 
     def __init__(self, cdll: C.CDLL):
         self.dll = L = cdll
@@ -167,6 +173,10 @@ class Api:
         L.jb_set_obs_stack.argtypes = [vp, C.c_int32, C.c_int32, c_int32_p, C.c_int32]
         L.jb_get_obs_stack.argtypes = [vp, c_double_p]
         L.jb_device_obs_views.argtypes = [vp, C.POINTER(vp), C.POINTER(vp)]
+        L.jb_set_mahony_filter_full.argtypes = [vp, C.c_double, C.c_double, C.c_int32, C.c_int32, C.c_int32]
+        L.jb_set_body_observer.argtypes = [vp, C.c_int32, C.c_double, C.c_int32]
+        L.jb_get_observers.argtypes = [vp, c_double_p]
+        L.jb_device_observer_views.argtypes = [vp, C.POINTER(vp)]
 
     def check(self, rc: int) -> None:
         if rc != JB_OK:
@@ -409,6 +419,37 @@ class BatchedEngine:
         """gym_jiminy's `MahonyFilter` observer on the device (exact_init, no twist removal); `kp=None` disables it."""
         self._api.check(self._api.dll.jb_set_mahony_filter(self._h, -1.0 if kp is None else float(kp), float(ki)))
 
+    def set_mahony_filter_full(self, kp: Optional[float] = 1.0, ki: float = 0.1, exact_init: bool = True,
+                               ignore_twist: bool = False, compute_rpy: bool = False) -> None:
+        """`MahonyFilter` with the reference's options: `exact_init=False` starts from the measured accelerometer
+        (the true orientation in free fall), `ignore_twist` removes the twist after every iteration, `compute_rpy`
+        fills the roll-pitch-yaw of `get_observers`.  `kp=None` disables the filter and the body observer."""
+        self._api.check(self._api.dll.jb_set_mahony_filter_full(self._h, -1.0 if kp is None else float(kp), float(ki),
+                                                                int(bool(exact_init)), int(bool(ignore_twist)),
+                                                                int(bool(compute_rpy))))
+
+    def set_body_observer(self, enable: bool = True, twist_time_constant: Optional[float] = None,
+                          compute_rpy: bool = True) -> None:
+        """gym_jiminy's `BodyObserver` after the Mahony filter: `twist_time_constant` None keeps the filter's twist, 0
+        removes it, > 0 re-estimates it with a leaky integrator.  Only between episodes (BadControlFlow while envs
+        run)."""
+        tc = float("nan") if twist_time_constant is None else float(twist_time_constant)
+        self._api.check(self._api.dll.jb_set_body_observer(self._h, int(bool(enable)), tc, int(bool(compute_rpy))))
+
+    def get_observers(self) -> np.ndarray:
+        """[n_env, nimu, OBSV_N]: MahonyFilter roll-pitch-yaw, BodyObserver quaternion, roll-pitch-yaw, angular velocity
+        and twist angle (BadControlFlow when the filter runs its default path only)."""
+        nimu = self.robot.sensor_layout()["ImuSensor"][2]
+        out = np.zeros((self.n_env, nimu, OBSV_N))
+        self._api.check(self._api.dll.jb_get_observers(self._h, dptr(out)))
+        return out
+
+    def device_observer_views(self) -> int:
+        """Device pointer of the observer record [n_env, nimu, OBSV_N]; 0 when there is none."""
+        o = C.c_void_p()
+        self._api.check(self._api.dll.jb_device_observer_views(self._h, C.byref(o)))
+        return o.value or 0
+
     def get_mahony_filter(self) -> np.ndarray:
         """[n_env, nimu, 10]: quaternion estimate (x, y, z, w), gyro bias estimate, unbiased angular velocity."""
         nimu = self.robot.sensor_layout()["ImuSensor"][2]
@@ -437,7 +478,7 @@ class BatchedEngine:
             return self.nm
         if leaf == STACK_PD_STATE:
             return 2 * self.nm
-        return 4 * self.robot.sensor_layout()["ImuSensor"][2]
+        return (4 if leaf in (STACK_MAHONY, STACK_BODY_QUAT) else 3) * self.robot.sensor_layout()["ImuSensor"][2]
 
     def get_obs_stack(self) -> np.ndarray:
         """The stacked frames [n_env, num_stack, frame width], oldest first (BadControlFlow when stacking is off)."""

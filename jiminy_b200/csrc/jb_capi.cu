@@ -59,6 +59,7 @@ struct JbBatch {
     double* d_springs = nullptr;
     double *d_pd = nullptr, *d_cmd_torque = nullptr, *d_pdf = nullptr, *d_pdf_state = nullptr, *d_mahony = nullptr;
     double *d_pdf_snap = nullptr, *d_mahony_snap = nullptr;
+    double *d_obsv = nullptr, *d_obsv_snap = nullptr;   // observer outputs beyond the MahonyFilter state, hand-off copies
     double* d_qbounds = nullptr;   // [2][nq] q_lower, q_upper (input checks of jb_start_device)
     // device PDAdapter (jb_set_pd_adapter)
     int32_t ad_order = -1, ad_instantaneous = 0;
@@ -539,6 +540,7 @@ int jb_batch_create(const JbModelDesc* m, const JbOptions* opt, int32_t n_env, i
     cudaMemcpyAsync(b->d_status, st.data(), N * sizeof(int32_t), cudaMemcpyHostToDevice, b->stream);
     kp.rint = d_rint; kp.rdbl = d_rdbl; kp.cslots = d_cs; kp.imu_placement = d_imu; kp.springs = nullptr;
     kp.pd_gains = nullptr; kp.cmd_torque = b->d_cmd_torque; kp.pdf = nullptr; kp.pdf_state = nullptr; kp.pdf_safety = 0; kp.mahony = nullptr; kp.mahony_kp = 1.0; kp.mahony_ki = 0.1;
+    kp.obsv = nullptr; kp.obsv_snap = nullptr; kp.mahony_exact_init = 1; kp.mahony_ignore_twist = 0; kp.mahony_rpy = 0; kp.body_on = 0;
     kp.q = b->d_q; kp.v = b->d_v; kp.a = b->d_a; kp.sched = b->d_sched; kp.iters = b->d_iters; kp.status = b->d_status;
     kp.command = b->d_cmd; kp.sensors = b->d_sensors; kp.qv_out = b->d_qv;
     kp.q_in = b->d_qin; kp.v_in = b->d_vin; kp.q_bounds = b->d_qbounds;
@@ -1232,10 +1234,28 @@ int jb_pd_adapter_device(JbBatch* b, const double* action_dev, double step_dt) {
     return JB_OK;
 }
 
-int jb_set_mahony_filter(JbBatch* b, double kp, double ki) {
+// The observer record (refresh_observers) exists when the filter leaves its default path or the body observer runs.
+static int update_observers(JbBatch* b) {
+    KParams& kp = b->kp;
+    const bool on = kp.mahony != nullptr && (!kp.mahony_exact_init || kp.mahony_ignore_twist || kp.mahony_rpy || kp.body_on);
+    if (!on) { kp.obsv = nullptr; kp.obsv_snap = nullptr; return JB_OK; }
+    if (!b->d_obsv) {
+        const size_t n = static_cast<size_t>(b->n_env) * b->nimu * OBSV_N;
+        int rc = dev_alloc(b, &b->d_obsv, n);
+        if (!rc) rc = dev_alloc(b, &b->d_obsv_snap, n);
+        if (rc) return rc;
+        CU(cudaStreamSynchronize(b->stream));
+    }
+    kp.obsv = b->d_obsv; kp.obsv_snap = b->d_obsv_snap;
+    return JB_OK;
+}
+
+int jb_set_mahony_filter(JbBatch* b, double kp, double ki) { return jb_set_mahony_filter_full(b, kp, ki, 1, 0, 0); }
+
+int jb_set_mahony_filter_full(JbBatch* b, double kp, double ki, int32_t exact_init, int32_t ignore_twist, int32_t compute_rpy) {
     if (!b) return fail(JB_ERR_INVALID_ARGUMENT, "null argument");
     CU(cudaSetDevice(b->device));
-    if (kp < 0.0) { b->kp.mahony = nullptr; return JB_OK; }
+    if (kp < 0.0) { b->kp.mahony = nullptr; b->kp.body_on = 0; return update_observers(b); }
     if (!b->nimu) return fail(JB_ERR_INVALID_ARGUMENT, "the robot has no IMU sensor");
     if (b->nimu > 1) return fail(JB_ERR_NOT_IMPLEMENTED, "the device Mahony filter handles one IMU per robot");
     if (!(b->kp.opt.sensors_update_period > 2.3e-16)) return fail(JB_ERR_NOT_IMPLEMENTED, "the Mahony filter needs a discrete sensorsUpdatePeriod");
@@ -1248,6 +1268,55 @@ int jb_set_mahony_filter(JbBatch* b, double kp, double ki) {
         CU(cudaStreamSynchronize(b->stream));
     }
     b->kp.mahony = b->d_mahony; b->kp.mahony_snap = b->d_mahony_snap; b->kp.mahony_kp = kp; b->kp.mahony_ki = ki;
+    b->kp.mahony_exact_init = exact_init != 0; b->kp.mahony_ignore_twist = ignore_twist != 0; b->kp.mahony_rpy = compute_rpy != 0;
+    return update_observers(b);
+}
+
+int jb_set_body_observer(JbBatch* b, int32_t enable, double twist_time_constant, int32_t compute_rpy) {
+    if (!b) return fail(JB_ERR_INVALID_ARGUMENT, "null argument");
+    if (b->any_started) return fail(JB_ERR_BAD_CONTROL_FLOW, "Simulation already running. Please stop it before configuring the body observer.");
+    if (!enable) { b->kp.body_on = 0; return update_observers(b); }
+    if (!b->kp.mahony) return fail(JB_ERR_INVALID_ARGUMENT, "the body observer needs the Mahony filter (jb_set_mahony_filter_full)");
+    const bool none = std::isnan(twist_time_constant);
+    if (!none && (twist_time_constant < 0.0 || std::isinf(twist_time_constant)))
+        return fail(JB_ERR_INVALID_ARGUMENT, "twist_time_constant must be NaN (None), 0 or finite and positive");
+    CU(cudaSetDevice(b->device));
+    // q_rel: matrices_to_quat (utils/math.py:307-350) of the IMU frame's rotation in its parent body (row-major)
+    double P[12];
+    CU(cudaMemcpyAsync(P, b->kp.imu_placement, sizeof P, cudaMemcpyDeviceToHost, b->stream));
+    CU(cudaStreamSynchronize(b->stream));
+    const double* R = P;
+    double t, o4[4];
+    if (R[8] < 0) {
+        if (R[0] > R[4]) { t = 1 + R[0] - R[4] - R[8]; o4[0] = t; o4[1] = R[3] + R[1]; o4[2] = R[2] + R[6]; o4[3] = R[7] - R[5]; }
+        else { t = 1 - R[0] + R[4] - R[8]; o4[0] = R[3] + R[1]; o4[1] = t; o4[2] = R[7] + R[5]; o4[3] = R[2] - R[6]; }
+    } else {
+        if (R[0] < -R[4]) { t = 1 - R[0] - R[4] + R[8]; o4[0] = R[2] + R[6]; o4[1] = R[7] + R[5]; o4[2] = t; o4[3] = R[3] - R[1]; }
+        else { t = 1 + R[0] + R[4] + R[8]; o4[0] = R[7] - R[5]; o4[1] = R[2] - R[6]; o4[2] = R[3] - R[1]; o4[3] = t; }
+    }
+    const double d = 2 * std::sqrt(t);
+    KParams& kp = b->kp;
+    for (int e = 0; e < 4; ++e) kp.body_qrel[e] = o4[e] / d;
+    kp.body_on = 1;
+    kp.body_remove_twist = !none;
+    kp.body_update_twist = !none && twist_time_constant > 0.0;
+    kp.body_tc_inv = kp.body_update_twist ? 1.0 / twist_time_constant : 0.0;
+    kp.body_rpy = compute_rpy != 0;
+    return update_observers(b);
+}
+
+int jb_get_observers(JbBatch* b, double* out) {
+    if (!b || !out) return fail(JB_ERR_INVALID_ARGUMENT, "null argument");
+    if (!b->kp.obsv) return fail(JB_ERR_BAD_CONTROL_FLOW, "no observer record: the Mahony filter runs its default path only");
+    CU(cudaSetDevice(b->device));
+    CU(cudaMemcpyAsync(out, b->d_obsv, sizeof(double) * b->n_env * b->nimu * OBSV_N, cudaMemcpyDeviceToHost, b->stream));
+    CU(cudaStreamSynchronize(b->stream));
+    return JB_OK;
+}
+
+int jb_device_observer_views(JbBatch* b, double** observers) {
+    if (!b) return fail(JB_ERR_INVALID_ARGUMENT, "null argument");
+    if (observers) *observers = b->kp.obsv;
     return JB_OK;
 }
 
@@ -1299,8 +1368,17 @@ int jb_set_obs_stack(JbBatch* b, int32_t num_stack, int32_t skip_frames_ratio, c
             if (id == JB_STACK_PD_ACTION) { lf.src = b->d_cmd; lf.stride = nm; lf.w = nm; }
             else { lf.src = b->d_pdf_state; lf.stride = 3 * nm; lf.w = 2 * nm; }
         } else {
+            // MahonyFilter state [nimu][10] (quaternion, bias, omega) and observer record [nimu][OBSV_N]
             if (!b->kp.mahony) return fail(JB_ERR_INVALID_ARGUMENT, "stacked MahonyFilter leaf: the filter is not enabled (jb_set_mahony_filter)");
-            lf.kind = STACK_QUAT; lf.src = b->d_mahony; lf.stride = b->nimu; lf.w = 4 * b->nimu;
+            const bool body = id >= JB_STACK_BODY_QUAT;
+            if (body && !b->kp.body_on) return fail(JB_ERR_INVALID_ARGUMENT, "stacked BodyObserver leaf: the observer is not enabled (jb_set_body_observer)");
+            if ((id == JB_STACK_MAHONY_RPY && !b->kp.mahony_rpy) || (id == JB_STACK_BODY_RPY && !b->kp.body_rpy))
+                return fail(JB_ERR_INVALID_ARGUMENT, "stacked roll-pitch-yaw leaf: compute_rpy is off");
+            static const int kOff[7] = {0, 7, OBSV_MAHONY_RPY, 4, OBSV_BODY_QUAT, OBSV_BODY_RPY, OBSV_BODY_OMEGA};
+            const int j = id - JB_STACK_MAHONY;
+            const bool rec = id == JB_STACK_MAHONY_RPY || body;
+            lf.kind = STACK_IMU_REC; lf.src = rec ? b->d_obsv : b->d_mahony; lf.rw = rec ? OBSV_N : 10; lf.off = kOff[j];
+            lf.stride = b->nimu; lf.w = (id == JB_STACK_MAHONY || id == JB_STACK_BODY_QUAT ? 4 : 3) * b->nimu;
         }
         w += lf.w;
     }

@@ -52,14 +52,18 @@ struct SensorDesc {
 };
 
 // One stacked observation leaf (jb_set_obs_stack): `w` doubles per frame, copied from the env's row of `src`
-// (src[env * stride + off + k]); STACK_T: the time of the refresh, src unused; STACK_QUAT: the quaternions of the
-// MahonyFilter state [n_env][nimu][10], field-major (k = field * nimu + imu, `stride` = nimu)
-enum : int32_t { STACK_ROW = 0, STACK_T = 1, STACK_QUAT = 2 };
-constexpr int STACK_MAX_LEAVES = 9;
+// (src[env * stride + off + k]); STACK_T: the time of the refresh, src unused; STACK_IMU_REC: w / nimu consecutive
+// fields from `off` of a per-IMU record of `rw` doubles ([n_env][nimu][rw]: the MahonyFilter state, the observer
+// outputs), field-major (k = field * nimu + imu, `stride` = nimu)
+enum : int32_t { STACK_ROW = 0, STACK_T = 1, STACK_IMU_REC = 2 };
+constexpr int STACK_MAX_LEAVES = 15;
 struct StackLeaf {
     const double* src;
-    int32_t kind, stride, off, w;
+    int32_t kind, stride, off, w, rw;
 };
+
+// Per-IMU record of the observer outputs beyond the MahonyFilter state ([n_env][nimu][OBSV_N], jb_get_observers)
+enum : int32_t { OBSV_MAHONY_RPY = 0, OBSV_BODY_QUAT = 3, OBSV_BODY_RPY = 7, OBSV_BODY_OMEGA = 10, OBSV_TWIST = 13, OBSV_N = 14 };
 
 struct KParams {
     int32_t n_env, n_pad;
@@ -224,6 +228,13 @@ struct KParams {
     int32_t* stk_n_snap;           // [n_env]
     int32_t stk_num, stk_skip, stk_w, stk_nleaf;
     StackLeaf stk_leaf[STACK_MAX_LEAVES];
+    // MahonyFilter options beyond its default path and the BodyObserver (refresh_observers); obsv null = neither
+    double* obsv;                  // [n_env][nimu][OBSV_N]
+    double* obsv_snap;             // [n_env][nimu][OBSV_N] at the top of a hot-path pass (restored on hand-off)
+    int32_t mahony_exact_init, mahony_ignore_twist, mahony_rpy;
+    int32_t body_on, body_remove_twist, body_update_twist, body_rpy;
+    double body_tc_inv;            // 1 / twist_time_constant
+    double body_qrel[4];           // the IMU frame's rotation in its parent body (matrices_to_quat), one IMU per robot
 };
 
 // Launch parameters live in constant memory (uniform constant-bank operands in every device
@@ -3304,6 +3315,128 @@ JB_DI void mahony_update(double* ms, V3 gyro, V3 acc) {
     }
 }
 
+// swing_from_vector (utils/math.py:1066-1137) on one column of a [4][nimu] batch: the "smallest" rotation taking
+// (v_x, v_y, v_z) to e_z.  The singular branch (v_z near -1) is the reference's per-column recursion, so its quaternion
+// gets the first-order renormalisation twice (once in the recursive call, once in the batched one).
+JB_DI void swing_from_vector(const double v_x, const double v_y, const double v_z, double* q) {
+    const double thr = 1e-5;   // TWIST_SWING_SINGULAR_THR
+    auto renormalise = [&]() {
+        const double s = (3.0 - (((q[0] * q[0] + q[1] * q[1]) + q[2] * q[2]) + q[3] * q[3])) / 2;
+        q[0] *= s; q[1] *= s; q[2] *= s; q[3] *= s;
+    };
+    if (v_z < -1.0 + thr) {
+        const double eps_thr = sqrt(thr);
+        const bool eps_x = -thr < v_x && v_x < thr, eps_y = -thr < v_y && v_y < thr;
+        double ratio = 0.0;
+        bool eps_ratio = false;
+        if (eps_x && !eps_y) { ratio = v_x / v_y; eps_ratio = -eps_thr < ratio && ratio < eps_thr; }
+        else if (eps_y && !eps_x) { ratio = v_y / v_x; eps_ratio = -eps_thr < ratio && ratio < eps_thr; }
+        const double w_2 = (1.0 + fmax(v_z, -1.0)) / 2.0;
+        if (eps_x && eps_y) { q[0] = 0.0; q[1] = sqrt(1.0 - w_2); }
+        else if (eps_ratio && eps_x) {
+            q[0] = -sqrt(1.0 - w_2) * (1 - 0.5 * (ratio * ratio));
+            q[1] = sqrt(1.0 - w_2) * (ratio - 0.5 * (ratio * ratio * ratio));
+        } else if (eps_ratio && eps_y) {
+            q[0] = -sqrt(1.0 - w_2) * (ratio - 0.5 * (ratio * ratio * ratio));
+            q[1] = sqrt(1.0 - w_2) * (1 - 0.5 * (ratio * ratio));
+        } else {
+            const double rx = v_x / v_y, ry = v_y / v_x;
+            q[0] = -sqrt((1.0 - w_2) / (1 + rx * rx));
+            q[1] = sqrt((1.0 - w_2) / (1 + ry * ry));
+        }
+        q[2] = 0.0;
+        q[3] = sqrt(w_2);
+        renormalise();
+    } else {
+        const double s = sqrt(2.0 * (1.0 + v_z));
+        q[0] = v_y / s; q[1] = -v_x / s; q[2] = 0.0; q[3] = s / 2;
+    }
+    renormalise();
+}
+
+// remove_twist_from_quat (utils/math.py:1203-1246): compute_tilt_from_quat, then swing_from_vector, in place
+JB_DI void remove_twist_from_quat(double* q) {
+    const double q_x = q[0], q_y = q[1], q_z = q[2], q_w = q[3];
+    swing_from_vector(2 * (q_x * q_z - q_y * q_w), 2 * (q_y * q_z + q_w * q_x), 1 - 2 * (q_x * q_x + q_y * q_y), q);
+}
+
+// quat_to_rpy (utils/math.py:159-197), with its first-order normalisation and its pitch through atan2 of two roots.
+// Not inlined: refresh_observers calls it twice, and each copy would carry three atan2.
+__device__ __noinline__ void quat_to_rpy(const double* q, double* rpy) {
+    const double q_xx = q[0] * q[0], q_xy = q[0] * q[1], q_xw = q[0] * q[3], q_yy = q[1] * q[1], q_yz = q[1] * q[2];
+    const double q_zz = q[2] * q[2], q_zw = q[2] * q[3], q_ww = q[3] * q[3];
+    const double norm_2_inv = (3.0 - (((q_xx + q_yy) + q_zz) + q_ww)) / 2;
+    const double q_yw = q[1] * q[3] * norm_2_inv, q_xz = q[0] * q[2] * norm_2_inv;
+    rpy[0] = atan2(2 * (q_xw + q_yz), 1.0 - 2 * (q_xx + q_yy));
+    rpy[1] = -3.141592653589793 / 2 + 2 * atan2(sqrt(1.0 + 2 * (q_yw - q_xz)), sqrt(1.0 - 2 * (q_yw - q_xz)));
+    rpy[2] = atan2(2 * (q_zw + q_xy), 1.0 - 2 * (q_yy + q_zz));
+}
+
+// The MahonyFilter options beyond its default path (blocks/mahony_filter.py:337-393) and the BodyObserver
+// (blocks/body_orientation_observer.py:211-266) at one observer refresh of the env, after the filter's own update and on
+// the measured row.  At a (re)start: exact_init = false replaces the exact start by the swing of the measured
+// accelerometer unless the robot is in free fall (every component below 0.1 g), with no iteration and no twist removal;
+// after an iteration: ignore_twist.  Then the filter's rpy, and the body observer's refresh, which the reference also
+// applies once at reset (update_twist included, with the full observer period, from a zero twist).
+__device__ __noinline__ void refresh_observers(const Ctx c, const bool at_start) {
+    jb_syncwarp(c);   // the filter's update of this refresh is complete (on the IMU record's owner lane or lane 0)
+    if (c.sub == 0) {
+        const JbSensorLayout& lay = KP->lay;
+        const double* mrow = KP->sensors + static_cast<size_t>(c.env) * lay.width;
+        const int n = KP->nimu;
+        for (int k = 0; k < n; ++k) {
+            double* ms = KP->mahony + (static_cast<size_t>(c.env) * n + k) * 10;
+            double* os = KP->obsv + (static_cast<size_t>(c.env) * n + k) * OBSV_N;
+            if (at_start) {
+                if (!KP->mahony_exact_init) {
+                    const double a_x = mrow[lay.imu_offset + 3 * n + k], a_y = mrow[lay.imu_offset + 4 * n + k];
+                    const double a_z = mrow[lay.imu_offset + 5 * n + k];
+                    const double g_thr = 0.1 * 9.81;   // 0.1 * EARTH_SURFACE_GRAVITY
+                    if (!(fabs(a_x) < g_thr && fabs(a_y) < g_thr && fabs(a_z) < g_thr)) {
+                        const double nrm = sqrt(a_x * a_x + a_y * a_y + a_z * a_z);
+                        swing_from_vector(a_x / nrm, a_y / nrm, a_z / nrm, ms);
+                    }
+                }
+            } else if (KP->mahony_ignore_twist) remove_twist_from_quat(ms);
+            if (KP->mahony_rpy) quat_to_rpy(ms, os + OBSV_MAHONY_RPY);
+            if (!KP->body_on) continue;
+            // quat_multiply(q_imu, q_rel, is_right_conjugate=True) (utils/math.py:553-627): its sign convention
+            // negates the real part of q_rel, so the result is -(q_imu * conj(q_rel)), as in the reference
+            const double* r = KP->body_qrel;
+            double* bq = os + OBSV_BODY_QUAT;
+            const double lx = ms[0], ly = ms[1], lz = ms[2], lw = ms[3];
+            bq[0] = ((lw * r[0] + (-lx) * r[3]) + ly * r[2]) - lz * r[1];
+            bq[1] = ((lw * r[1] - lx * r[2]) + (-ly) * r[3]) + lz * r[0];
+            bq[2] = ((lw * r[2] + lx * r[1]) - ly * r[0]) + (-lz) * r[3];
+            bq[3] = (((-lw) * r[3] - lx * r[0]) - ly * r[1]) - lz * r[2];
+            // quat_apply(q_rel, omega_imu) (utils/math.py:646-707)
+            const double q_xx = r[0] * r[0], q_xy = r[0] * r[1], q_xz = r[0] * r[2], q_xw = r[0] * r[3];
+            const double q_yy = r[1] * r[1], q_yz = r[1] * r[2], q_yw = r[1] * r[3];
+            const double q_zz = r[2] * r[2], q_zw = r[2] * r[3], q_ww = r[3] * r[3];
+            const double x = ms[7], y = ms[8], z = ms[9];
+            double* bo = os + OBSV_BODY_OMEGA;
+            bo[0] = (x * (((q_xx + q_ww) - q_yy) - q_zz) + y * (2 * q_xy - 2 * q_zw)) + z * (2 * q_xz + 2 * q_yw);
+            bo[1] = (x * (2 * q_zw + 2 * q_xy) + y * (((q_ww - q_xx) + q_yy) - q_zz)) + z * (-2 * q_xw + 2 * q_yz);
+            bo[2] = (x * (-2 * q_yw + 2 * q_xz) + y * (2 * q_xw + 2 * q_yz)) + z * (((q_ww - q_xx) - q_yy) + q_zz);
+            if (KP->body_remove_twist) remove_twist_from_quat(bq);
+            if (KP->body_update_twist) {
+                // update_twist (blocks/body_orientation_observer.py:26-72): leaky integrator of the twist angle
+                const double dt = KP->opt.sensors_update_period;
+                double tw = at_start ? 0.0 : os[OBSV_TWIST];
+                const double b_x = bq[0], b_y = bq[1], b_w = bq[3];
+                const double dtwist = ((-b_y) * bo[0] + b_x * bo[1]) / b_w + bo[2];
+                tw *= fmax(0.0, 1.0 - KP->body_tc_inv * dt);
+                tw += dtwist * dt;
+                double p_z, p_w;
+                sincos(0.5 * tw, &p_z, &p_w);
+                bq[0] = p_w * b_x - p_z * b_y; bq[1] = p_z * b_x + p_w * b_y; bq[2] = p_z * b_w; bq[3] = p_w * b_w;
+                os[OBSV_TWIST] = tw;
+            }
+            if (KP->body_rpy) quat_to_rpy(bq, os + OBSV_BODY_RPY);
+        }
+    }
+}
+
 // StackObservation.refresh_observation (wrappers/observation_stack.py:221-254) at one observer refresh of the env, on the
 // measured row and the block states this refresh left.  The frames hold what the wrapper's stacked observation holds:
 // the latest frame always the current value, a shift (the refresh right after a stack update) drops the oldest frame,
@@ -3335,7 +3468,7 @@ __device__ __noinline__ void stack_observation(const Ctx c, const bool at_start,
             for (int k = c.sub; k < lf.w; k += L) {
                 double x;
                 if (lf.kind == STACK_T) x = t_obs;
-                else if (lf.kind == STACK_QUAT) x = lf.src[(static_cast<size_t>(c.env) * lf.stride + k % lf.stride) * 10 + k / lf.stride];
+                else if (lf.kind == STACK_IMU_REC) x = lf.src[(static_cast<size_t>(c.env) * lf.stride + k % lf.stride) * lf.rw + lf.off + k / lf.stride];
                 else x = lf.src[static_cast<size_t>(c.env) * lf.stride + lf.off + k];
                 last[o + k] = x;
             }
@@ -3516,6 +3649,7 @@ __device__ __noinline__ void write_sensors(const Ctx c, const bool at_start, con
                               mk(mrow[lay.imu_offset + 3 * n + k], mrow[lay.imu_offset + 4 * n + k], mrow[lay.imu_offset + 5 * n + k]));
         }
     }
+    if (KP->obsv != nullptr) refresh_observers(c, at_start);
     if (KP->stk != nullptr) stack_observation(c, at_start, t_obs, step_dt);
 }
 

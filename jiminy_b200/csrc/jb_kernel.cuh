@@ -252,6 +252,13 @@ __device__ __noinline__ void snapshot_blocks(const Ctx c, const int L, const boo
         double* live = KP->mahony + static_cast<size_t>(c.env) * n;
         double* snap = KP->mahony_snap + static_cast<size_t>(c.env) * n;
         for (size_t k = c.sub; k < n; k += L) { if (restore) live[k] = snap[k]; else snap[k] = live[k]; }
+        if (KP->obsv != nullptr) {
+            // observer outputs and the body observer's twist (refresh_observers)
+            const size_t m = OBSV_N * static_cast<size_t>(KP->nimu);
+            double* lo = KP->obsv + static_cast<size_t>(c.env) * m;
+            double* so = KP->obsv_snap + static_cast<size_t>(c.env) * m;
+            for (size_t k = c.sub; k < m; k += L) { if (restore) lo[k] = so[k]; else so[k] = lo[k]; }
+        }
     }
     if (KP->sp_on) {
         // sensor measurement pipeline: sample counts and generator states (ring slots written by the aborted pass are rewritten)

@@ -17,12 +17,13 @@ the flat sensor row.
 from __future__ import annotations
 
 import functools
-from typing import Any, Dict, Optional, Sequence, Tuple
+from typing import Any, Dict, Optional, Sequence, Tuple, Union
 
 import numpy as np
 
-from . import compositions, core, model_randomisation, scenarios, sensor_randomisation
+from . import compositions, core, model_randomisation, observers, scenarios, sensor_randomisation
 from .observation_stack import StackObservation
+from .observers import BodyObserver, MahonyFilter
 from .disturbance import from_std_ratio
 from .model import RobotTable
 
@@ -63,12 +64,14 @@ class without_plain_pd:
 
 def configure_pd_blocks(env, kp, kd, joint_position_margin: float, joint_velocity_limit: float,
                         joint_acceleration_limit: Optional[float], safety: Optional[Dict[str, float]], order: int,
-                        joint_velocity_deadband: float, mahony: Optional[Tuple[float, float]], training: bool) -> Optional[np.ndarray]:
-    """`MotorSafetyLimit` -> `PDController` -> `MahonyFilter` on `env.engine` from the constructor arguments of
-    `PDControlBatchedEnv`, with the bounds the reference's block constructors derive from them
+                        joint_velocity_deadband: float, mahony, training: bool,
+                        body_observer: Optional[BodyObserver] = None) -> Optional[np.ndarray]:
+    """`MotorSafetyLimit` -> `PDController` -> `MahonyFilter` (-> `BodyObserver`) on `env.engine` from the constructor
+    arguments of `PDControlBatchedEnv`, with the bounds the reference's block constructors derive from them
     (blocks/proportional_derivative_controller.py:301-450, :560-640; blocks/motor_safety_limit.py:112-175).  Sets
-    `env.command_state_lower / upper` [3, nmotors], `env.action_low / high` and `env._mahony`; returns the `PDAdapter`'s
-    motor velocity dead band (None in training mode)."""
+    `env.command_state_lower / upper` [3, nmotors], `env.action_low / high`, `env._mahony` and, for the object form of
+    `mahony`, `env._observers` (the filter and the body observer, else None); returns the `PDAdapter`'s motor velocity
+    dead band (None in training mode)."""
     rob, nm, dt = env.robot, env.robot.nmotors, env.step_dt
     kp, kd = np.broadcast_to(kp, (nm,)).astype(np.float64), np.broadcast_to(kd, (nm,)).astype(np.float64)
     ratio = np.array([m.reduction for m in rob.motors])
@@ -92,7 +95,15 @@ def configure_pd_blocks(env, kp, kd, joint_position_margin: float, joint_velocit
                           q_lo + ratio * safety["soft_position_margin"], q_hi - ratio * safety["soft_position_margin"],
                           np.minimum(v_hw, ratio * safety["soft_velocity_max"])])
     env.engine.set_pd_controller_full(kp, kd, env.command_state_lower, env.command_state_upper, table)
-    if mahony is not None:
+    env._observers = None
+    if isinstance(mahony, MahonyFilter):
+        mahony.configure(env.engine)
+        if body_observer is not None:
+            body_observer.configure(env.engine)
+        env._observers = (mahony, body_observer)
+    elif body_observer is not None:
+        raise ValueError("body_observer needs the MahonyFilter object form of `mahony`")
+    elif mahony is not None:
         env.engine.set_mahony_filter(*mahony)
     env._mahony = mahony is not None
     if order not in (0, 1):
@@ -180,7 +191,8 @@ class BatchedJiminyEnv:
         if stack is None:
             return
         shapes = self._obs_shapes()
-        leaves = stack.resolve(shapes)
+        obs_blocks = getattr(self, "_observers", None)
+        leaves = stack.resolve(shapes, observers.stack_leaves(*obs_blocks) if obs_blocks is not None else None)
         self.engine.set_obs_stack(stack.num_stack, stack.skip_frames_ratio, [code for _, code in leaves])
         col = 0
         for path, code in leaves:
@@ -332,8 +344,13 @@ def pd_obs_shapes(env, shapes: Dict[str, Any]) -> Dict[str, Any]:
     """The leaves a PD env adds to the observation tree of `_obs_shapes`, in the order of its `_observation`."""
     nm = env.robot.nmotors
     shapes["states"]["pd_controller"] = (2, nm)
-    if env._mahony:
-        shapes["features"] = {"mahony_filter": (4, env.robot.sensor_layout()["ImuSensor"][2])}
+    nimu = env.robot.sensor_layout()["ImuSensor"][2]
+    if env._observers is not None:
+        extra = observers.observation_shapes(*env._observers, nimu)
+        shapes["states"].update(extra["states"])
+        shapes["features"] = extra["features"]
+    elif env._mahony:
+        shapes["features"] = {"mahony_filter": (4, nimu)}
     if env.augment_observation:
         shapes["actions"] = {"pd_controller": (nm,)}
     return shapes
@@ -349,13 +366,18 @@ class PDControlBatchedEnv(BatchedJiminyEnv):
     blocks/motor_safety_limit.py:112-175).  The action is the adapter's: target motor velocities (order 1) or
     positions (order 0) at the end of the step, within the controller's command-state bounds.
     `augment_observation=True` adds the controller's action, the target accelerations of the env-step
-    (`obs["actions"]["pd_controller"]`), as the reference's `ControlledJiminyEnv` does (bases/pipeline.py:1134-1141)."""
+    (`obs["actions"]["pd_controller"]`), as the reference's `ControlledJiminyEnv` does (bases/pipeline.py:1134-1141).
+    `mahony`: `(kp, ki)` for the filter's default path, observed as the quaternion array `features.mahony_filter`
+    [n_env, 4, nimu]; or a `jiminy_b200.observers.MahonyFilter`, observed with the reference's layout
+    (`features.<name> = {"quat", ["rpy"], "omega"}`, `states.<name> = {"bias"}`), which `body_observer` (a
+    `jiminy_b200.observers.BodyObserver`, `features.<name> = {"quat", ["rpy"], "omega"}`) needs."""
 
     def __init__(self, scenario: scenarios.Scenario, *, kp=None, kd=None, joint_position_margin: float = 0.0,
                  joint_velocity_limit: float = float("inf"), joint_acceleration_limit: Optional[float] = None,
                  safety: Optional[Dict[str, float]] = None, order: int = 1, joint_velocity_deadband: float = 0.0,
-                 is_instantaneous: bool = False, mahony: Optional[Tuple[float, float]] = None, training: bool = True,
-                 augment_observation: bool = False, stack: Optional[StackObservation] = None, **kw):
+                 is_instantaneous: bool = False, mahony: Union[None, Tuple[float, float], MahonyFilter] = None,
+                 training: bool = True, augment_observation: bool = False, stack: Optional[StackObservation] = None,
+                 body_observer: Optional[BodyObserver] = None, **kw):
         from .blocks import PDAdapter
         kp, kd = pd_gains(scenario, kp, kd)
         self.training = training
@@ -363,7 +385,7 @@ class PDControlBatchedEnv(BatchedJiminyEnv):
         with without_plain_pd(scenario):          # the base class must not install the plain PD law
             super().__init__(scenario, **kw)
         deadband = configure_pd_blocks(self, kp, kd, joint_position_margin, joint_velocity_limit, joint_acceleration_limit,
-                                       safety, order, joint_velocity_deadband, mahony, training)
+                                       safety, order, joint_velocity_deadband, mahony, training, body_observer)
         self._setup_stack(stack)
         self.adapter = PDAdapter(self.engine, self.command_state_lower, self.command_state_upper, order=order,
                                  is_instantaneous=is_instantaneous, velocity_deadband=deadband, step_dt=self.step_dt)
@@ -374,7 +396,12 @@ class PDControlBatchedEnv(BatchedJiminyEnv):
     def _plain_observation(self) -> Dict[str, Any]:
         obs = super()._plain_observation()
         obs["states"]["pd_controller"] = self.engine.get_pd_controller_state()[:, :2]       # PDController.get_state (:488-489)
-        if self._mahony:
+        if self._observers is not None:
+            record = self.engine.get_observers() if observers.has_record(*self._observers) else None
+            extra = observers.observation(*self._observers, self.engine.get_mahony_filter(), record, np.ascontiguousarray)
+            obs["states"].update(extra["states"])
+            obs["features"] = extra["features"]
+        elif self._mahony:
             obs["features"] = {"mahony_filter": np.swapaxes(self.engine.get_mahony_filter()[:, :, :4], 1, 2)}   # [n, 4, n_imu]
         if self.augment_observation:
             obs["actions"] = {"pd_controller": self.engine.get_efforts()[2]}      # the block's action (pipeline.py:1134-1141)

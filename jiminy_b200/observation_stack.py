@@ -8,7 +8,9 @@ arguments against an env's observation tree and reads the wrapper entry of a ref
 
 Each stacked leaf of the observation is replaced by its frames `[n_env, num_stack, *leaf shape]`, oldest first.  The
 leaves that can be stacked are `t`, a sensor-type block of `measurements`, `actions.pd_controller` (PD envs built with
-`augment_observation=True`), `states.pd_controller` and `features.mahony_filter`; any other selected leaf, the agent's
+`augment_observation=True`), `states.pd_controller`, `features.mahony_filter` and the leaves of the observer blocks
+(`jiminy_b200.observers`: the filter's `quat`, `rpy`, `omega` and state `bias`, the body observer's `quat`, `rpy` and
+`omega`); any other selected leaf, the agent's
 `states.agent.q / v` included (and so the reference's default of every leaf), raises NotImplementedError.
 """
 from __future__ import annotations
@@ -62,18 +64,21 @@ class StackObservation:
         self.nested_filter_keys = None if nested_filter_keys is None else \
             [(k,) if isinstance(k, (str, int)) else tuple(k) for k in nested_filter_keys]
 
-    def resolve(self, obs: Dict[str, Any]) -> List[Tuple[Tuple[str, ...], int]]:
-        """(path, leaf code) of every stacked leaf of the observation `obs`, in its order (`observation_stack.py:96-105`)."""
+    def resolve(self, obs: Dict[str, Any], extra: Optional[Dict[Tuple[str, ...], int]] = None
+                ) -> List[Tuple[Tuple[str, ...], int]]:
+        """(path, leaf code) of every stacked leaf of the observation `obs`, in its order (`observation_stack.py:96-105`);
+        `extra` maps the paths of the env's observer leaves (`jiminy_b200.observers.stack_leaves`) to their codes."""
+        known = LEAVES if not extra else {**LEAVES, **extra}
         paths = leaf_paths(obs)
         keys = self.nested_filter_keys if self.nested_filter_keys is not None else [(k,) for k in obs]
         chosen = [p for p in paths if any(p[:len(e)] == e for e in keys)]
         if not chosen:
             raise ValueError("At least one observation leaf must be stacked.")
         for p in chosen:
-            if p not in LEAVES:
+            if p not in known:
                 raise NotImplementedError(f"stacking the observation leaf {'.'.join(map(str, p))} is not supported on the "
-                                          f"batched envs (supported: {', '.join('.'.join(k) for k in LEAVES)})")
-        return [(p, LEAVES[p]) for p in chosen]
+                                          f"batched envs (supported: {', '.join('.'.join(k) for k in known)})")
+        return [(p, known[p]) for p in chosen]
 
 
 def from_config(layers_config: Sequence[dict]) -> Optional[StackObservation]:

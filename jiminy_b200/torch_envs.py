@@ -66,7 +66,7 @@ from typing import Any, Dict, Optional, Tuple, Union
 import numpy as np
 import torch
 
-from . import core, envs, scenarios
+from . import core, envs, observers, scenarios
 from .parallel import _DevArray
 
 _CTYPES = {torch.float64: C.c_double, torch.int32: C.c_int32}
@@ -159,6 +159,8 @@ class DeviceBatchedEnv(envs.BatchedJiminyEnv):
         self._pd_state = self._view(pd_state, (n, 3, self.robot.nmotors)) if pd_state else None
         nimu = self.robot.sensor_layout()["ImuSensor"][2]
         self._mahony_state = self._view(mahony, (n, nimu, 10)) if mahony else None
+        record = eng.device_observer_views()
+        self._observer_record = self._view(record, (n, nimu, core.OBSV_N)) if record else None
         stack, command = eng.device_obs_views()
         self._command = self._view(command, (n, self.robot.nmotors)) if self.robot.nmotors else None
         self._stack_frames = self._view(stack, (n,) + eng.stack_shape) if self._stack_leaves else None
@@ -388,14 +390,14 @@ class DeviceBatchedEnv(envs.BatchedJiminyEnv):
 
 class DevicePDControlBatchedEnv(DeviceBatchedEnv):
     """`PDControlBatchedEnv` (MotorSafetyLimit -> PDController -> PDAdapter -> MahonyFilter) with the adapter on the device
-    as well: same constructor arguments and bounds (`envs.configure_pd_blocks`), `augment_observation` and `stack`
-    included, plus those of `DeviceBatchedEnv`."""
+    as well: same constructor arguments and bounds (`envs.configure_pd_blocks`), `augment_observation`, `stack`, the
+    `MahonyFilter` object form of `mahony` and `body_observer` included, plus those of `DeviceBatchedEnv`."""
 
     def __init__(self, scenario: scenarios.Scenario, *, kp=None, kd=None, joint_position_margin: float = 0.0,
                  joint_velocity_limit: float = float("inf"), joint_acceleration_limit: Optional[float] = None,
                  safety: Optional[Dict[str, float]] = None, order: int = 1, joint_velocity_deadband: float = 0.0,
-                 is_instantaneous: bool = False, mahony: Optional[Tuple[float, float]] = None, training: bool = True,
-                 augment_observation: bool = False, stack=None, **kw):
+                 is_instantaneous: bool = False, mahony=None, training: bool = True,
+                 augment_observation: bool = False, stack=None, body_observer=None, **kw):
         kp, kd = envs.pd_gains(scenario, kp, kd)
         self.training = training
         self.augment_observation = augment_observation
@@ -403,7 +405,7 @@ class DevicePDControlBatchedEnv(DeviceBatchedEnv):
         with envs.without_plain_pd(scenario):
             envs.BatchedJiminyEnv.__init__(self, scenario, **kw)
         deadband = envs.configure_pd_blocks(self, kp, kd, joint_position_margin, joint_velocity_limit, joint_acceleration_limit,
-                                            safety, order, joint_velocity_deadband, mahony, training)
+                                            safety, order, joint_velocity_deadband, mahony, training, body_observer)
         self.engine.set_pd_adapter(order, is_instantaneous, deadband)
         self._setup_stack(stack)
         self._init_device(reset_states, torch_device, kw.get("api_"))
@@ -414,7 +416,12 @@ class DevicePDControlBatchedEnv(DeviceBatchedEnv):
     def _plain_observation(self) -> Dict[str, Any]:
         obs = super()._plain_observation()
         obs["states"]["pd_controller"] = self._pd_state[:, :2].clone()      # PDController.get_state (:488-489)
-        if self._mahony:
+        if self._observers is not None:
+            extra = observers.observation(*self._observers, self._mahony_state, self._observer_record,
+                                          lambda x: x.clone(memory_format=torch.contiguous_format))
+            obs["states"].update(extra["states"])
+            obs["features"] = extra["features"]
+        elif self._mahony:
             obs["features"] = {"mahony_filter": self._mahony_state[:, :, :4].transpose(1, 2).clone()}   # [n, 4, n_imu]
         if self.augment_observation:
             obs["actions"] = {"pd_controller": self._command.clone()}         # the block's action (pipeline.py:1134-1141)

@@ -48,16 +48,24 @@ num_stack NUM, skip_frames_ratio SKIP), alternating in one process, `max(--alter
 `t`, `measurements.ImuSensor` and 12 doubles of motor data, 19 doubles per frame: `measurements.EffortSensor` on the
 plain-PD ANYmal and anymal_flexible envs, the PDController's action (`augment_observation=True`) on Atlas.
 
+`--observers` times the device loop with the MahonyFilter on its default path (exact start, no twist removal, no rpy)
+against the full observer set (`jiminy_b200.observers`: `MahonyFilter(exact_init=False, ignore_twist=True,
+compute_rpy=True)` and `BodyObserver(twist_time_constant=0.3)`), alternating in one process, `max(--alternate, 1)` rounds:
+the cost of the observers' refreshes inside the step kernel and of their observation leaves.  Atlas flattens the
+filter's quaternion in both; the plain-PD ANYmal and anymal_flexible envs get the filter on their engine in both (their
+observation does not include it).
+
     python tools/bench_pipeline.py [--robot atlas|anymal|anymal_flexible] [--loop host|device] [--alternate R]
                                    [--n-env 4096] [--steps 10] [--warmup 3] [--duration-max 0.4] [--disturbance R]
                                    [--sensors R] [--model R] [--model-bias S] [--restart bank|sample] [--compositions]
-                                   [--stack NUM,SKIP]
+                                   [--stack NUM,SKIP] [--observers]
 """
 import argparse
 import json
 import os
 import sys
 import time
+from typing import Optional
 
 import numpy as np
 
@@ -72,8 +80,9 @@ KEYS = [("states", "pd_controller"), ("measurements", "EncoderSensor"), ("featur
 
 def make_env(n_env: int, api_=None, robot: str = "atlas", loop: str = "host", duration_max: float = 20.0,
              disturbance: float = 0.0, sensors: float = 0.0, model: float = 0.0, restart: str = "bank",
-             model_bias: float = 0.0, compositions: bool = False, stack=None):
+             model_bias: float = 0.0, compositions: bool = False, stack=None, observers=None):
     from jiminy_b200 import envs, scenarios
+    from jiminy_b200.observers import BodyObserver, MahonyFilter
     from jiminy_b200.observation_stack import StackObservation
     from jiminy_b200.model_randomisation import BIAS_OPTIONS
     ratio = {k: r for k, r in (("disturbance", disturbance), ("sensors", sensors), ("model", model)) if r > 0}
@@ -92,13 +101,21 @@ def make_env(n_env: int, api_=None, robot: str = "atlas", loop: str = "host", du
             kw["augment_observation"] = True
     if robot in ("anymal", "anymal_flexible"):
         from jiminy_b200.torch_envs import DeviceBatchedEnv
-        return (DeviceBatchedEnv if loop == "device" else envs.BatchedJiminyEnv)(scenarios.make(robot, n_env, seed=0), **kw)
+        env = (DeviceBatchedEnv if loop == "device" else envs.BatchedJiminyEnv)(scenarios.make(robot, n_env, seed=0), **kw)
+        if observers is not None:
+            env.engine.set_mahony_filter_full(1.0, 0.1, exact_init=not observers, ignore_twist=observers, compute_rpy=observers)
+            if observers:
+                env.engine.set_body_observer(True, 0.3, True)
+        return env
+    if observers:
+        kw["mahony"] = MahonyFilter(MAHONY_KP, MAHONY_KI, exact_init=False, ignore_twist=True, compute_rpy=True)
+        kw["body_observer"] = BodyObserver(twist_time_constant=0.3)
     from jiminy_b200.torch_envs import DevicePDControlBatchedEnv
     sc = scenarios.make(robot, n_env, seed=0, contact_model="constraint", solver="euler_explicit", dt_max=0.005)
     return (DevicePDControlBatchedEnv if loop == "device" else envs.PDControlBatchedEnv)(
         sc, joint_position_margin=0.0, joint_velocity_limit=MOTOR_VELOCITY_MAX, joint_acceleration_limit=MOTOR_ACCELERATION_MAX,
         safety=dict(kp=1.0 / MOTOR_POSITION_MARGIN, kd=MOTOR_VELOCITY_SAFE_GAIN, soft_position_margin=0.0, soft_velocity_max=MOTOR_VELOCITY_MAX),
-        order=1, mahony=(MAHONY_KP, MAHONY_KI), **kw)
+        order=1, **{"mahony": (MAHONY_KP, MAHONY_KI), **kw})
 
 
 def representative_compositions(step_dt: float) -> dict:
@@ -133,10 +150,11 @@ def gpu_info() -> dict:
 
 def run(n_env: int, steps: int, warmup: int, api_=None, robot: str = "atlas", loop: str = "host",
         duration_max: float = 0.4, disturbance: float = 0.0, sensors: float = 0.0, model: float = 0.0,
-        restart: str = "bank", model_bias: float = 0.0, compositions: bool = False, stack=None) -> dict:
+        restart: str = "bank", model_bias: float = 0.0, compositions: bool = False, stack=None, observers=None) -> dict:
     import torch
     from jiminy_b200.envs import flatten_observation
-    env = make_env(n_env, api_, robot, loop, duration_max, disturbance, sensors, model, restart, model_bias, compositions, stack)
+    env = make_env(n_env, api_, robot, loop, duration_max, disturbance, sensors, model, restart, model_bias, compositions, stack,
+                   observers)
     device = loop == "device"
     on_gpu = device and env.torch_device.type == "cuda"
     nm = env.robot.nmotors
@@ -148,6 +166,8 @@ def run(n_env: int, steps: int, warmup: int, api_=None, robot: str = "atlas", lo
     if device:
         acts = [torch.as_tensor(a, device=env.torch_device) for a in acts]
     keys = KEYS if robot == "atlas" else [("states", "agent", "q"), ("states", "agent", "v")]
+    if robot == "atlas" and observers:
+        keys = [("features", "mahony_filter", "quat") if k == ("features", "mahony_filter") else k for k in keys]
     low = {KEYS[0]: env.command_state_lower[:2]} if robot == "atlas" else None
     high = {KEYS[0]: env.command_state_upper[:2]} if robot == "atlas" else None
 
@@ -179,7 +199,7 @@ def run(n_env: int, steps: int, warmup: int, api_=None, robot: str = "atlas", lo
             f"contacts, euler_explicit 5 ms" if robot == "atlas" else
             f"{robot} PD standing (plain PD law), spring-damper contacts, runge_kutta_4 1 ms, per-step position targets")
     out = {"metric": "env_steps_per_sec", "unit": "env-steps/s", "value": n_env * steps / dt, "ms_per_step": 1e3 * dt / steps,
-           "loop": loop, "restart": restart, "stack": stack, "robot": robot, "disturbance": disturbance, "sensors": sensors, "model": model, "model_bias": model_bias, "n_env": n_env, "steps": steps, "warmup": warmup,
+           "loop": loop, "restart": restart, "stack": stack, "observers": observers, "robot": robot, "disturbance": disturbance, "sensors": sensors, "model": model, "model_bias": model_bias, "n_env": n_env, "steps": steps, "warmup": warmup,
            "timing": "host clock around env.step + flatten_observation, ending in a device synchronise",
            "config": {"workload": f"{desc}, {n_env} envs, step_dt {env.step_dt}, simulation_duration_max {duration_max}",
                       "env": type(env).__name__, "lane_plan": env.engine.describe(), "observation_width": int(flat.shape[1])},
@@ -208,15 +228,17 @@ def alternate(rounds: int, **kw) -> dict:
     return out
 
 
-def alternate_randomisation(rounds: int, ratios: dict, loops, **kw) -> dict:
+def alternate_randomisation(rounds: int, ratios: dict, loops, off: Optional[dict] = None, **kw) -> dict:
     """Each loop with the randomisation of `ratios` ({"disturbance": r}, {"sensors": r}, {"model": r},
-    {"model_bias": s}, {"restart": "sample"}, {"compositions": True} or {"stack": (num, skip)}) off and on, `rounds` times in this process, alternating; env-steps/s and spread."""
+    {"model_bias": s}, {"restart": "sample"}, {"compositions": True}, {"stack": (num, skip)} or {"observers": True}) off and
+    on, `rounds` times in this process, alternating; env-steps/s and spread.  `off` keyword arguments are given to the off
+    runs."""
     name = "_".join(ratios)
     runs = {(loop, on): [] for loop in loops for on in (False, True)}
     for _ in range(rounds):
         for loop in loops:
             for on in (False, True):
-                runs[(loop, on)].append(run(loop=loop, **(ratios if on else {}), **kw))
+                runs[(loop, on)].append(run(loop=loop, **(ratios if on else off or {}), **kw))
     out = {"metric": "env_steps_per_sec", "unit": "env-steps/s", "robot": kw.get("robot", "atlas"), "rounds": rounds}
     for (loop, on), rs in runs.items():
         v = sorted(x["value"] for x in rs)
@@ -245,6 +267,7 @@ if __name__ == "__main__":
     ap.add_argument("--restart", choices=("bank", "sample"), default="bank")
     ap.add_argument("--compositions", action="store_true")
     ap.add_argument("--stack", type=str, default=None, metavar="NUM,SKIP")
+    ap.add_argument("--observers", action="store_true")
     a = ap.parse_args()
     kw = dict(n_env=a.n_env, steps=a.steps, warmup=a.warmup, robot=a.robot, duration_max=a.duration_max)
     ratios = {k: r for k, r in (("disturbance", a.disturbance), ("sensors", a.sensors), ("model", a.model)) if r > 0}
@@ -252,6 +275,11 @@ if __name__ == "__main__":
         num, skip = (int(x) for x in a.stack.split(","))
         res = alternate_randomisation(max(a.alternate, 1), {"stack": (num, skip)}, ("device",), **ratios, **kw)
         off, on = res["device_stack_off"], res["device_stack_on"]
+        res["added_ms_per_env_step"] = on["ms_per_step_median"] - off["ms_per_step_median"]
+    elif a.observers:
+        res = alternate_randomisation(max(a.alternate, 1), {"observers": True}, ("device",), off={"observers": False},
+                                      **ratios, **kw)
+        off, on = res["device_observers_off"], res["device_observers_on"]
         res["added_ms_per_env_step"] = on["ms_per_step_median"] - off["ms_per_step_median"]
     elif a.compositions:
         res = alternate_randomisation(max(a.alternate, 1), {"compositions": True}, ("device",), **ratios, **kw)
